@@ -94,6 +94,18 @@ typedef struct {
     uint32_t n_mod, n_canon, n_other, n_delete, n_filtered, n_diff, n_nocall;
 } mkp_row;                /* 40 bytes */
 
+/* ---- output row of `pileup-hemi` == DuplexPatternCounts of one pattern (src/pileup/duplex.rs:33-57), integers only -------
+ * valid_coverage = count + n_other_pattern; the percentage is formatted by the host. Eleven u32 fields: no count fits in
+ * less, so the row is 44 bytes. */
+#define MKP_HEMI_CANONICAL 0u     /* code_pos / code_neg of a canonical call ('-')                                            */
+typedef struct {
+    uint32_t pos;             /* + strand motif position                                                                  */
+    uint32_t code_pos;        /* call on the + strand at pos: MKP_HEMI_CANONICAL, char code point, or 0x80000000|ChEBI   */
+    uint32_t code_neg;        /* call on the - strand at the motif's partner position, same encoding                     */
+    uint32_t primary_base;    /* 0..3 = A C G T: the read base at pos                                                     */
+    uint32_t count, n_other_pattern, n_canonical, n_delete, n_fail, n_diff, n_nocall;
+} mkp_hemi_row;           /* 44 bytes */
+
 typedef struct {          /* per-chunk counters, filled by mkp_pileup_* */
     uint64_t n_rows;
     uint64_t n_hot;           /* positions that received a counter slot            */
@@ -129,6 +141,20 @@ int  mkp_pileup_resident(mkp_ctx* ctx, mkp_stats* stats);
 /* Copy the rows of the last mkp_pileup_resident to host memory owned by ctx
  * (sorted by position, then strand '+' < '-', then code). */
 int  mkp_fetch_rows(mkp_ctx* ctx, const mkp_row** rows, size_t* n_rows);
+
+/* `modkit pileup-hemi` (src/pileup/duplex.rs) over the resident chunk: duplex pattern counts per + strand motif position.
+ * The chunk's focus_pos bitmap holds the + strand positions of the (palindromic) motif; focus_neg is not read. Every call
+ * record inside [start, end) of the chunk is kept, so the chunk must reach `partner_offset` past its focus positions on either
+ * side (partner = p + partner_offset = reverse offset - forward offset; negative for e.g. GATC 3). interval_starts[0 ..
+ * n_intervals) (host memory, non-decreasing, the first at or before the first focus position): the reference intervals the chunk
+ * holds; a read without usable mod info counts one NoCall in each of them. mkp_params.numeric_mode 1 = --combine-mods,
+ * 2 = --ignore. MKP_FUSED / MKP_TILE do not apply to this pass. */
+int  mkp_hemi_resident(mkp_ctx* ctx, const uint32_t* interval_starts, uint32_t n_intervals, int32_t partner_offset,
+                       mkp_stats* stats);
+
+/* Copy the rows of the last mkp_hemi_resident to host memory owned by ctx (sorted by position, then primary base, then
+ * (code_pos, code_neg) with MKP_HEMI_CANONICAL first). */
+int  mkp_fetch_hemi_rows(mkp_ctx* ctx, const mkp_hemi_row** rows, size_t* n_rows);
 
 /* upload + pileup + fetch in one call: the drop-in for process_region_batch on host buffers. */
 int  mkp_pileup_chunk(mkp_ctx* ctx, const mkp_chunk* host_chunk, const mkp_row** rows, size_t* n_rows,

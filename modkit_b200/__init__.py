@@ -46,16 +46,24 @@ ROW_DTYPE = np.dtype([("pos", "<u4"), ("code", "<u4"), ("strand", "u1"), ("prima
                       ("n_mod", "<u4"), ("n_canon", "<u4"), ("n_other", "<u4"), ("n_delete", "<u4"),
                       ("n_filtered", "<u4"), ("n_diff", "<u4"), ("n_nocall", "<u4")])
 assert ROW_DTYPE.itemsize == 40
+# mkp_hemi_row (include/mkp.h): one `pileup-hemi` pattern row; code_pos / code_neg == HEMI_CANONICAL is '-'
+HEMI_CANONICAL = 0
+HEMI_ROW_DTYPE = np.dtype([("pos", "<u4"), ("code_pos", "<u4"), ("code_neg", "<u4"), ("primary_base", "<u4"), ("count", "<u4"),
+                           ("n_other_pattern", "<u4"), ("n_canonical", "<u4"), ("n_delete", "<u4"), ("n_fail", "<u4"),
+                           ("n_diff", "<u4"), ("n_nocall", "<u4")])
+assert HEMI_ROW_DTYPE.itemsize == 44
 
 MKP_SYMBOLS = ["mkp_create", "mkp_bind_host_thread", "mkp_destroy", "mkp_last_error", "mkp_set_params", "mkp_upload_chunk", "mkp_pileup_resident",
                "mkp_fetch_rows", "mkp_pileup_chunk", "mkp_sample_histogram", "mkp_sample_summary", "mkp_algorithmic_bytes", "mkp_kernel_launches",
-               "mkp_device_memory", "mkp_bam_load", "mkp_bam_load_range", "mkp_bam_load_range_fd", "mkp_bam_records", "mkp_bam_chunk", "mkp_bam_tags", "mkp_bam_inflated", "mkp_fetch_chunk"]
+               "mkp_device_memory", "mkp_bam_load", "mkp_bam_load_range", "mkp_bam_load_range_fd", "mkp_bam_records", "mkp_bam_chunk", "mkp_bam_tags", "mkp_bam_inflated", "mkp_fetch_chunk",
+               "mkp_hemi_resident", "mkp_fetch_hemi_rows"]
 MKH_SYMBOLS = ["mkh_pileup_main", "mkh_bam_open", "mkh_bam_close", "mkh_bam_n_refs", "mkh_bam_ref_name", "mkh_bam_ref_len",
                "mkh_bam_n_mapped", "mkh_bam_n_records", "mkh_pack_region", "mkh_packed_free", "mkh_packed_n_reads",
                "mkh_packed_hdrs", "mkh_packed_heap", "mkh_packed_heap_bytes", "mkh_packed_algorithmic_bytes", "mkh_format_rows",
                "mkh_motif_focus", "mkh_bam_open_device", "mkh_device_chunk", "mkh_bam_ingest_ms", "mkh_bam_total_records",
                "mkh_f32_display", "mkh_bam_partition_key", "mkh_bam_n_ranges", "mkh_pileup_main_sharded", "mkh_shard_plan",
-               "mkh_bam_open_device_pieces", "mkh_bam_fetch", "mkh_summary_main", "mkh_sample_probs_main", "mkh_partition_key_of_cells", "mkh_bam_index_n_mapped", "mkh_pct2"]
+               "mkh_bam_open_device_pieces", "mkh_bam_fetch", "mkh_summary_main", "mkh_sample_probs_main", "mkh_partition_key_of_cells", "mkh_bam_index_n_mapped", "mkh_pct2",
+               "mkh_pileup_hemi_main", "mkh_pileup_hemi_main_sharded"]
 
 ALLREDUCE_FN = C.CFUNCTYPE(C.c_int, C.POINTER(C.c_uint64), C.c_size_t, C.c_void_p)
 
@@ -85,6 +93,9 @@ def load_library(build_if_missing=True):
     lib.mkp_upload_chunk.argtypes = [C.c_void_p, C.POINTER(Chunk)]
     lib.mkp_pileup_resident.argtypes = [C.c_void_p, C.POINTER(Stats)]
     lib.mkp_fetch_rows.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]
+    lib.mkp_hemi_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_int32, C.POINTER(Stats)]
+    lib.mkp_fetch_hemi_rows.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]
+    lib.mkh_pileup_hemi_main_sharded.argtypes = [C.c_int, C.POINTER(C.c_char_p), C.c_int, C.c_int, ALLREDUCE_FN, C.c_void_p, C.POINTER(C.c_double)]
     lib.mkp_pileup_chunk.argtypes = [C.c_void_p, C.POINTER(Chunk), C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.POINTER(Stats)]
     lib.mkp_sample_histogram.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
     lib.mkp_sample_summary.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -166,6 +177,14 @@ def pileup_main(args):
     return lib.mkh_pileup_main(len(args), argv)
 
 
+def pileup_hemi_main(args):
+    """In-process `modkit pileup-hemi <args>` (output to -o FILE, else stdout); returns the exit code (0 ok, 1 runtime error,
+    2 usage)."""
+    lib = load_library()
+    argv = (C.c_char_p * len(args))(*[str(a).encode() for a in args])
+    return lib.mkh_pileup_hemi_main(len(args), argv)
+
+
 def bind_host_thread(device):
     """Pin this thread (and threads started later) to the CPUs of the device's NUMA node. Returns 0 when bound."""
     return load_library().mkp_bind_host_thread(int(device))
@@ -193,15 +212,15 @@ def torch_allreduce(device=None):
     return fn
 
 
-def pileup_main_sharded(args, rank, world, allreduce):
-    """One rank of an interval-sharded `modkit pileup <args>` (every rank passes the same args plus its own --device).
-    `allreduce(buf, n, user) -> 0` sums a u64 vector over the ranks in place (see torch_allreduce).
-    Returns (exit code, stats dict)."""
+def pileup_main_sharded(args, rank, world, allreduce, hemi=False):
+    """One rank of an interval-sharded `modkit pileup <args>` (every rank passes the same args plus its own --device);
+    hemi=True: `modkit pileup-hemi <args>`. `allreduce(buf, n, user) -> 0` sums a u64 vector over the ranks in place (see
+    torch_allreduce). Returns (exit code, stats dict)."""
     lib = load_library()
     argv = (C.c_char_p * len(args))(*[str(a).encode() for a in args])
     cb = ALLREDUCE_FN(allreduce) if allreduce is not None else C.cast(None, ALLREDUCE_FN)
     st = (C.c_double * 20)()
-    rc = lib.mkh_pileup_main_sharded(len(args), argv, rank, world, cb, None, st)
+    rc = (lib.mkh_pileup_hemi_main_sharded if hemi else lib.mkh_pileup_main_sharded)(len(args), argv, rank, world, cb, None, st)
     keys = ["total_s", "load_s", "thresholds_s", "gpu_s", "write_s", "rows_total", "positions_total", "rows_rank",
             "threshold_A", "threshold_C", "threshold_G", "threshold_T", "sampler_fetch_s", "intervals_s", "pack_s", "kernel_ms", "slice_s", "pass_s", "rowcopy_s"]
     return rc, dict(zip(keys, [float(x) for x in st]))
@@ -467,6 +486,22 @@ class Context:
             return np.zeros(0, dtype=ROW_DTYPE)
         buf = (C.c_uint8 * (40 * n.value)).from_address(rows.value)
         return np.frombuffer(buf, dtype=ROW_DTYPE)   # view of ctx-owned pinned memory; copy() to keep
+
+    def hemi_resident(self, interval_starts, partner_offset):
+        """`pileup-hemi` pass over the resident chunk (its focus_pos = the + strand motif positions)."""
+        starts = np.ascontiguousarray(interval_starts, dtype=np.uint32)
+        st = Stats()
+        self._check(self._lib.mkp_hemi_resident(self._h, starts.ctypes.data, len(starts), int(partner_offset), C.byref(st)))
+        return st
+
+    def fetch_hemi_rows(self):
+        rows = C.c_void_p()
+        n = C.c_size_t()
+        self._check(self._lib.mkp_fetch_hemi_rows(self._h, C.byref(rows), C.byref(n)))
+        if not n.value:
+            return np.zeros(0, dtype=HEMI_ROW_DTYPE)
+        buf = (C.c_uint8 * (HEMI_ROW_DTYPE.itemsize * n.value)).from_address(rows.value)
+        return np.frombuffer(buf, dtype=HEMI_ROW_DTYPE).copy()
 
     def pileup_chunk(self, packed):
         ch = packed.chunk()

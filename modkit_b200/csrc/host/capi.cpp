@@ -18,6 +18,16 @@ int mkh_pileup_main(int argc, const char* const* argv) {
     return 0;
 }
 
+// In-process `modkit pileup-hemi` (src/pileup/subcommand.rs:825-1514): duplex pattern counts, to -o FILE or stdout.
+int mkh_pileup_hemi_main(int argc, const char* const* argv) {
+    PileupOptions o;
+    std::string err;
+    if (!parse_pileup_args(argc, argv, &o, &err, true)) { fprintf(stderr, "error: %s\n", err.c_str()); return 2; }
+    RunSummary s;
+    if (run_pileup_devices(o, &s, &err)) { fprintf(stderr, "> Error! %s\n", err.c_str()); return 1; }
+    return 0;
+}
+
 // In-process `modkit summary` / `modkit sample-probs` (SURVEY 8f-3): the report goes to stdout, or to --out FILE.
 static int sample_main(int argc, const char* const* argv, bool summary) {
     SampleOptions o;
@@ -38,10 +48,10 @@ int mkh_sample_probs_main(int argc, const char* const* argv) { return sample_mai
 // sizes (u64[world + 2]); with --include-unmapped a third, one-word exchange precedes them.
 // out_stats (optional, double[20]): total_s, load_s, thresholds_s, gpu_s, write_s, rows (all ranks), positions (all ranks), rows of this
 // rank, base thresholds A C G T (-1 = none), sampler fetch_s, intervals_s, pack_s, kernel_ms, slice_s, pass_s, rowcopy_s.
-int mkh_pileup_main_sharded(int argc, const char* const* argv, int rank, int world, int (*allreduce)(uint64_t*, size_t, void*), void* user, double* out_stats) {
+static int pileup_main_sharded(int argc, const char* const* argv, bool hemi, int rank, int world, int (*allreduce)(uint64_t*, size_t, void*), void* user, double* out_stats) {
     PileupOptions o;
     std::string err;
-    if (!parse_pileup_args(argc, argv, &o, &err)) { fprintf(stderr, "error: %s\n", err.c_str()); return 2; }
+    if (!parse_pileup_args(argc, argv, &o, &err, hemi)) { fprintf(stderr, "error: %s\n", err.c_str()); return 2; }
     if (rank < 0 || world < 1 || rank >= world || (world > 1 && !allreduce)) { fprintf(stderr, "error: bad rank/world\n"); return 2; }
     Collective c;
     c.rank = rank; c.world = world; c.allreduce_sum = allreduce; c.user = user;
@@ -54,6 +64,13 @@ int mkh_pileup_main_sharded(int argc, const char* const* argv, int rank, int wor
                      out_stats[12] = s.fetch_s; out_stats[13] = s.interval_s; out_stats[14] = s.pack_s; out_stats[15] = s.kernel_ms;
                      out_stats[16] = s.slice_s; out_stats[17] = s.pass_s; out_stats[18] = s.rowcopy_s; }
     return 0;
+}
+int mkh_pileup_main_sharded(int argc, const char* const* argv, int rank, int world, int (*allreduce)(uint64_t*, size_t, void*), void* user, double* out_stats) {
+    return pileup_main_sharded(argc, argv, false, rank, world, allreduce, user, out_stats);
+}
+// One rank of an interval-sharded `modkit pileup-hemi`: as mkh_pileup_main_sharded (the ranks need -o FILE).
+int mkh_pileup_hemi_main_sharded(int argc, const char* const* argv, int rank, int world, int (*allreduce)(uint64_t*, size_t, void*), void* user, double* out_stats) {
+    return pileup_main_sharded(argc, argv, true, rank, world, allreduce, user, out_stats);
 }
 
 // Shard plan of a BAM for `world` ranks (the cuts run_pileup uses; CPU only: header + index, no device): fills

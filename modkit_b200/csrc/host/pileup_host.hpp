@@ -663,6 +663,37 @@ inline void format_bed_row(const OutRow& o, const std::string& chrom, const BedF
     out->append(b0, (size_t)(p - b0));
 }
 
+// `pileup-hemi` row (src/writers.rs:185-255): name `{pos call},{neg call},{base}` ('-' = canonical), strand '.', percent of the
+// pattern among the base's patterns
+inline void format_hemi_row(const mkp_hemi_row& r, const std::string& chrom, bool mixed_delim, std::string* out) {
+    const uint32_t cov = r.count + r.n_other_pattern;
+    const char sp = mixed_delim ? ' ' : '\t';
+    char stack_buf[640];
+    std::string big;
+    char* b0 = stack_buf;
+    if (chrom.size() + 256 > sizeof stack_buf) { big.resize(chrom.size() + 256); b0 = &big[0]; }
+    char* p = b0;
+    auto code = [&](uint32_t c) {
+        if (c == MKP_HEMI_CANONICAL) *p++ = '-';
+        else if (c & 0x80000000u) p = put_u32(p, c & 0x7fffffffu);
+        else *p++ = (char)c;
+    };
+    memcpy(p, chrom.data(), chrom.size()); p += chrom.size();
+    *p++ = '\t'; p = put_u32(p, r.pos); *p++ = '\t'; p = put_u32(p, r.pos + 1); *p++ = '\t';
+    code(r.code_pos); *p++ = ','; code(r.code_neg); *p++ = ','; *p++ = "ACGT"[r.primary_base & 3];
+    *p++ = '\t'; p = put_u32(p, cov); memcpy(p, "\t.\t", 3); p += 3; p = put_u32(p, r.pos); *p++ = '\t'; p = put_u32(p, r.pos + 1);
+    memcpy(p, "\t255,0,0\t", 9); p += 9;
+    p = put_u32(p, cov); *p++ = sp;
+    // duplex.rs:44-46 and writers.rs:231: format!("{:.2}", count as f32 / valid_coverage as f32 * 100f32)
+    const float frac = (float)r.count / (float)cov;
+    volatile float pct = frac * 100.0f;
+    p = put_pct2(p, pct);
+    *p++ = sp; p = put_u32(p, r.count); *p++ = sp; p = put_u32(p, r.n_canonical); *p++ = sp; p = put_u32(p, r.n_other_pattern);
+    *p++ = sp; p = put_u32(p, r.n_delete); *p++ = sp; p = put_u32(p, r.n_fail); *p++ = sp; p = put_u32(p, r.n_diff);
+    *p++ = sp; p = put_u32(p, r.n_nocall); *p++ = '\n';
+    out->append(b0, (size_t)(p - b0));
+}
+
 // --bedgraph (src/writers.rs:318-381): `chrom start end fraction coverage`, one file per (partition, strand, code[, motif])
 inline const char* strand_label(char s) { return s == '+' ? "positive" : s == '-' ? "negative" : s == '.' ? "combined" : "_unknown"; }
 inline std::string bedgraph_label(const OutRow& o, const BedFormat& fmt) {

@@ -41,7 +41,26 @@ struct PileupOptions {
     bool quiet = false;
     uint32_t max_depth = 8000;         // --max-depth (src/pileup/subcommand.rs:117-121)
     std::vector<int> devices;          // --devices a,b,...: one interval shard per listed GPU (threads of this process)
+    bool hemi = false;                 // `modkit pileup-hemi`: duplex pattern counts at the + strand positions of one palindromic motif
 };
+
+// pileup-hemi's motif (src/pileup/subcommand.rs:1242-1272): exactly one, --cpg or --motif, and it must be a palindrome. Checked
+// before any device work, so argument errors need no GPU.
+inline MotifSpec hemi_motif(const PileupOptions& o) {
+    if (o.ref_fp.empty()) throw std::runtime_error("the following required arguments were not provided: --ref <REFERENCE_FASTA>");
+    if (o.cpg && !o.motif_parts.empty()) throw std::runtime_error("the argument '--cpg' cannot be used with '--motif <MOTIF> <MOTIF>'");
+    if (o.motif_parts.size() > 2) throw std::runtime_error("the argument '--motif <MOTIF> <MOTIF>' cannot be used multiple times");
+    if (!o.cpg && o.motif_parts.empty()) throw std::runtime_error("either --cpg or a --motif must be provided for pileup-hemi");
+    MotifSpec m;
+    if (o.cpg) m = parse_motif("CG", 0);
+    else {
+        const std::string& off = o.motif_parts[1];
+        if (off.empty() || off.find_first_not_of("0123456789") != std::string::npos) throw std::runtime_error("couldn't parse focus position, " + off);
+        m = parse_motif(o.motif_parts[0], std::stoi(off));
+    }
+    if (!m.palindromic) throw std::runtime_error("motif must be palindromic for pileup-hemi");
+    return m;
+}
 
 struct Region { std::string name; uint32_t start = 0, end = 0; };
 
@@ -761,6 +780,9 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
         trace_clock().epoch = t0;
         auto trace = [&](const char* what) { trace_clock().mark(coll.rank, what); };
         if (o.percentile > 1.0f) throw std::runtime_error("filter percentile must be <= 1.0");
+        MotifSpec hemi_m;
+        if (o.hemi) hemi_m = hemi_motif(o);
+        const int32_t hemi_partner = o.hemi ? hemi_m.rc_offset - hemi_m.offset : 0;     // MotifInfo::negative_strand_position
         // the device comes first: with the device ingest (default) the BAM is inflated and sliced on the GPU
         DeviceGuard dev;
         {
@@ -801,7 +823,7 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
             include.read(o.include_bed, name_to_tid);
             inc = &include;
         }
-        bool combine_strands = o.combine_strands;
+        bool combine_strands = o.combine_strands || o.hemi;        // pileup-hemi: the feeder runs in combine-strands mode
         if (combine_strands && !(o.cpg || !o.motif_parts.empty())) throw std::runtime_error("need to specify either --motif or --cpg to combine strands");
 
         mkp_params P;
@@ -821,7 +843,8 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
         std::vector<std::string> parts = o.motif_parts;
         MotifContext mc;
         bool have_motifs = false;
-        if (!parts.empty()) {
+        if (o.hemi) { mc.motifs.push_back(hemi_m); have_motifs = true; }
+        else if (!parts.empty()) {
             if (o.traditional) throw std::runtime_error("cannot use presets and motifs together");
             if (parts.size() % 2) throw std::runtime_error("illegal number of parts for motif");
             for (size_t i = 0; i < parts.size(); i += 2) for (size_t j = i + 2; j < parts.size(); j += 2)
@@ -1063,7 +1086,7 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
         // ---- two stages: a device thread selects the reads of chunk after chunk, slices them on the GPU, runs the pass and takes
         // the rows; this thread turns finished chunks into text (strand combining, formatting: parallel over intervals) and
         // writes them in order. The device works on chunk k + 1 while chunk k is being formatted.
-        struct ChunkOut { size_t i0 = 0, i1 = 0; std::string key_name; std::vector<mkp_row> rows; bool last = false; };
+        struct ChunkOut { size_t i0 = 0, i1 = 0; std::string key_name; std::vector<mkp_row> rows; std::vector<mkp_hemi_row> hemi_rows; bool last = false; };
         std::mutex q_mu;
         std::condition_variable q_cv;
         std::deque<ChunkOut> queue;
@@ -1115,6 +1138,10 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
                         const size_t i0 = wk.a, i1 = wk.b;
                         const uint32_t cs = ivs[i0].start, ce = ivs[i1 - 1].end;
                         if (ce <= cs || wk.recs.empty()) continue;
+                        // pileup-hemi: the call window reaches the partner of every motif position; the reads stay those of the intervals
+                        uint32_t wcs = cs, wce = ce;
+                        if (hemi_partner < 0) wcs = cs - std::min<uint32_t>(cs, (uint32_t)-hemi_partner);
+                        if (hemi_partner > 0) wce = (uint32_t)std::min<uint64_t>((uint64_t)ce + (uint32_t)hemi_partner, std::max(ce, bam.ref_lens[ivs[i0].tid]));
                         std::vector<RecRef>& all_recs = wk.recs;
                         // with --partition-tag one group per key (each an independent pileup: src/pileup/mod.rs:795-830), in key order
                         std::map<std::string, std::vector<RecRef>> groups;
@@ -1157,38 +1184,50 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
                             if (pc.recs.empty()) continue;
                             mkp_chunk ch;
                             memset(&ch, 0, sizeof ch);
-                            ch.start = cs; ch.end = ce; ch.hdrs = pc.hdrs.data(); ch.n_reads = (uint32_t)pc.hdrs.size(); ch.heap = pc.heap.data(); ch.heap_bytes = pc.heap.size();
-                            if (have_motifs || inc) { if (!focus_done) { focus_bitmaps(ivs, i0, i1, cs, ce, &fpos, &fneg); focus_done = true; } ch.focus_pos = fpos.data(); ch.focus_neg = fneg.data(); }
+                            ch.start = wcs; ch.end = wce; ch.hdrs = pc.hdrs.data(); ch.n_reads = (uint32_t)pc.hdrs.size(); ch.heap = pc.heap.data(); ch.heap_bytes = pc.heap.size();
+                            if (have_motifs || inc) { if (!focus_done) { focus_bitmaps(ivs, i0, i1, wcs, wce, &fpos, &fneg); focus_done = true; } ch.focus_pos = fpos.data(); ch.focus_neg = fneg.data(); }
                             const auto tb = clk::now();
                             S.pack_s += secs(ta, tb);
                             const mkp_row* rows = nullptr;
+                            const mkp_hemi_row* hemi_rows = nullptr;
                             size_t n_rows = 0;
                             mkp_stats st;
+                            auto hemi_pass = [&]() {
+                                std::vector<uint32_t> starts;
+                                for (size_t k = i0; k < i1; k++) starts.push_back(ivs[k].start);
+                                if (mkp_hemi_resident(dev.ctx, starts.data(), (uint32_t)starts.size(), hemi_partner, &st)) throw std::runtime_error(mkp_last_error(dev.ctx));
+                            };
                             if (bam.on_device) {
                                 // slice on the GPU (no packed chunk in host memory), then the same kernels
-                                device_chunk(bam, pc.recs, cs, ce, ch.focus_pos, ch.focus_neg);
+                                device_chunk(bam, pc.recs, wcs, wce, ch.focus_pos, ch.focus_neg);
                                 const auto t_s = clk::now();
                                 S.slice_s += secs(tb, t_s);
-                                if (mkp_pileup_resident(dev.ctx, &st)) throw std::runtime_error(mkp_last_error(dev.ctx));
+                                if (o.hemi) hemi_pass();
+                                else if (mkp_pileup_resident(dev.ctx, &st)) throw std::runtime_error(mkp_last_error(dev.ctx));
                                 const auto t_k = clk::now();
                                 S.pass_s += secs(t_s, t_k);
-                                if (mkp_fetch_rows(dev.ctx, &rows, &n_rows)) throw std::runtime_error(mkp_last_error(dev.ctx));
+                                if (o.hemi ? mkp_fetch_hemi_rows(dev.ctx, &hemi_rows, &n_rows) : mkp_fetch_rows(dev.ctx, &rows, &n_rows)) throw std::runtime_error(mkp_last_error(dev.ctx));
                                 S.rowcopy_s += secs(t_k, clk::now());
                                 if (want_alg_bytes) {
                                     pc.hdrs.resize(pc.recs.size());
                                     uint32_t nr = 0;
                                     if (mkp_fetch_chunk(dev.ctx, pc.hdrs.data(), &nr, nullptr, nullptr)) throw std::runtime_error(mkp_last_error(dev.ctx));
                                 }
+                            } else if (o.hemi) {
+                                if (mkp_upload_chunk(dev.ctx, &ch)) throw std::runtime_error(mkp_last_error(dev.ctx));
+                                hemi_pass();
+                                if (mkp_fetch_hemi_rows(dev.ctx, &hemi_rows, &n_rows)) throw std::runtime_error(mkp_last_error(dev.ctx));
                             } else if (mkp_pileup_chunk(dev.ctx, &ch, &rows, &n_rows, &st)) throw std::runtime_error(mkp_last_error(dev.ctx));
                             ChunkOut co;
                             co.i0 = i0; co.i1 = i1;
                             co.key_name = !partitioned ? std::string() : (grp.first == "\1" ? std::string("ungrouped") : grp.first);
                             { std::lock_guard<std::mutex> lk(q_mu); if (!spare_rows.empty()) { co.rows.swap(spare_rows.back()); spare_rows.pop_back(); } }
-                            co.rows.assign(rows, rows + n_rows);          // the context's row buffer is reused by the next chunk
+                            if (o.hemi) co.hemi_rows.assign(hemi_rows, hemi_rows + n_rows);
+                            else co.rows.assign(rows, rows + n_rows);          // the context's row buffer is reused by the next chunk
                             S.gpu_s += secs(tb, clk::now());
                             S.kernel_ms += st.kernel_ms[7];
                             S.reads_packed += pc.recs.size();
-                            S.algorithmic_bytes += (want_alg_bytes || !bam.on_device ? pc.algorithmic_bytes() : 0) + 40 * n_rows;
+                            S.algorithmic_bytes += (want_alg_bytes || !bam.on_device ? pc.algorithmic_bytes() : 0) + (o.hemi ? sizeof(mkp_hemi_row) : sizeof(mkp_row)) * n_rows;
                             S.chunks++;
                             push_out(std::move(co));
                         }
@@ -1219,7 +1258,8 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
             const auto tc = clk::now();
             const size_t i0 = co.i0, i1 = co.i1;
             const mkp_row* rows = co.rows.data();
-            const size_t n_rows = co.rows.size();
+            const size_t n_rows = o.hemi ? co.hemi_rows.size() : co.rows.size();
+            auto pos_of = [&](size_t j) { return o.hemi ? co.hemi_rows[j].pos : rows[j].pos; };
             const std::string& key_name = co.key_name;
             // rows are position sorted: every interval gets its slice; intervals are finished and formatted in parallel
             const std::string& chrom = bam.ref_names[ivs[i0].tid];
@@ -1227,9 +1267,9 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
             std::vector<size_t> rlo(n_iv + 1);
             {
                 size_t r0 = 0;
-                for (size_t i = i0; i < i1; i++) { while (r0 < n_rows && rows[r0].pos < ivs[i].start) r0++; rlo[i - i0] = r0; }
+                for (size_t i = i0; i < i1; i++) { while (r0 < n_rows && pos_of(r0) < ivs[i].start) r0++; rlo[i - i0] = r0; }
                 size_t r1 = rlo[n_iv - 1];
-                while (r1 < n_rows && rows[r1].pos < ivs[i1 - 1].end) r1++;
+                while (r1 < n_rows && pos_of(r1) < ivs[i1 - 1].end) r1++;
                 rlo[n_iv] = r1;
             }
             const int nt = std::max(1, std::min<int>(o.threads, (int)n_iv));
@@ -1250,7 +1290,12 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
                     for (size_t k = a; k < b; k++) {
                         const size_t r_end = k + 1 < n_iv ? std::max(rlo[k], rlo[k + 1]) : rlo[n_iv];
                         size_t r1 = rlo[k];
-                        while (r1 < r_end && rows[r1].pos < ivs[i0 + k].end) r1++;
+                        while (r1 < r_end && pos_of(r1) < ivs[i0 + k].end) r1++;
+                        if (o.hemi) {       // rows are final: one per (position, base, pattern), in output order
+                            for (size_t j = rlo[k]; j < r1; j++) format_hemi_row(co.hemi_rows[j], chrom, o.mixed, &parts[t]);
+                            part_rows[t] += r1 - rlo[k];
+                            continue;
+                        }
                         local.clear();
                         finish_interval_rows(ivs[i0 + k], rows + rlo[k], r1 - rlo[k], have_motifs ? &mc.motifs : nullptr, combine_strands, &local);
                         if (!to_dir) for (auto& orow : local) format_bed_row(orow, chrom, fmt, &parts[t]);
@@ -1427,14 +1472,20 @@ inline int run_pileup_devices(const PileupOptions& o, RunSummary* summary, std::
     return 0;
 }
 
-// clap-compatible subset of the `modkit pileup` flag surface (src/pileup/subcommand.rs:37-379)
-inline bool parse_pileup_args(int argc, const char* const* argv, PileupOptions* o, std::string* err) {
+// clap-compatible subset of the `modkit pileup` flag surface (src/pileup/subcommand.rs:37-379). hemi: `modkit pileup-hemi`
+// (src/pileup/subcommand.rs:825-1130): the same flags without --preset, --combine-strands, --bedgraph, --with-header, --prefix
+// and --partition-tag, one positional <IN_BAM>, output to -o/--out-bed or stdout.
+inline bool parse_pileup_args(int argc, const char* const* argv, PileupOptions* o, std::string* err, bool hemi = false) {
     std::vector<std::string> pos;
+    o->hemi = hemi;
     for (int i = 0; i < argc; i++) {
         const std::string a = argv[i];
         auto val = [&]() -> std::string { if (i + 1 >= argc) throw std::runtime_error("a value is required for '" + a + "' but none was supplied"); return argv[++i]; };
         try {
-            if (a == "-t" || a == "--threads") o->threads = std::stoi(val());
+            if (hemi && (a == "--preset" || a == "--combine-strands" || a == "--bedgraph" || a == "--header" || a == "--with-header" ||
+                         a == "--include_header" || a == "--prefix" || a == "--partition-tag")) { *err = "unexpected argument '" + a + "' found"; return false; }
+            if (hemi && (a == "-o" || a == "--out-bed")) o->out_bed = val();
+            else if (a == "-t" || a == "--threads") o->threads = std::stoi(val());
             else if (a == "-i" || a == "--interval-size") o->interval_size = (uint32_t)std::stoul(val());
             else if (a == "--region") o->region = val();
             else if (a == "--sample-region") o->sample_region = val();
@@ -1475,6 +1526,12 @@ inline bool parse_pileup_args(int argc, const char* const* argv, PileupOptions* 
             else if (a.size() > 1 && a[0] == '-') { *err = "unexpected argument '" + a + "' found"; return false; }
             else pos.push_back(a);
         } catch (const std::exception& e) { *err = e.what(); return false; }
+    }
+    if (hemi) {
+        if (pos.size() != 1) { *err = pos.empty() ? "the following required arguments were not provided: <IN_BAM>" : "unexpected argument '" + pos[1] + "' found"; return false; }
+        o->in_bam = pos[0];
+        if (o->out_bed.empty()) o->out_bed = "-";
+        return true;
     }
     if (pos.size() != 2) { *err = "the following required arguments were not provided: <IN_BAM> <OUT_BED>"; return false; }
     o->in_bam = pos[0]; o->out_bed = pos[1];

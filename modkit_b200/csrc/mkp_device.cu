@@ -91,6 +91,11 @@ struct mkp_ctx {
     std::vector<uint64_t> h_entry_off;
     mkp_row* h_rows_pinned = nullptr;
     size_t h_rows_pinned_cap = 0;
+    // pileup-hemi pass: interval starts, its own hot bitmap (k_resolve's marks) and focus rank (d_hot / d_hot_prefix hold the
+    // rank the fused pileup pass builds once per chunk), rows (device, host)
+    DevBuf d_iv_start, d_hemi_hot, d_hemi_prefix, d_hemi_rows;
+    size_t n_hemi_rows = 0;
+    std::vector<mkp_hemi_row> h_hemi_rows;
 };
 
 // d_small layout (u64 words): [0..31] states, [32] total_calls, [33] hist_inexact ; u32 view from byte 34*8: n_states, err, n_hot, n_rows
@@ -170,7 +175,8 @@ void mkp_destroy(mkp_ctx* ctx) {
                       &ctx->d_calls, &ctx->d_hot, &ctx->d_hot_prefix, &ctx->d_block_sums, &ctx->d_small, &ctx->d_scr_cq, &ctx->d_scr_cr, &ctx->d_slow,
                       &ctx->d_obs_word, &ctx->d_slots, &ctx->d_row_counts, &ctx->d_row_prefix, &ctx->d_rows, &ctx->d_hist, &ctx->d_take,
                       &ctx->d_file, &ctx->d_members, &ctx->d_bam, &ctx->d_seeds, &ctx->d_seg_counts, &ctx->d_seg_base, &ctx->d_recs, &ctx->d_ids, &ctx->d_plan,
-                      &ctx->d_need, &ctx->d_totals, &ctx->d_slab_work, &ctx->d_pscr, &ctx->d_inftab, &ctx->d_tiles, &ctx->d_order};
+                      &ctx->d_need, &ctx->d_totals, &ctx->d_slab_work, &ctx->d_pscr, &ctx->d_inftab, &ctx->d_tiles, &ctx->d_order,
+                      &ctx->d_iv_start, &ctx->d_hemi_hot, &ctx->d_hemi_prefix, &ctx->d_hemi_rows};
     for (auto* b : bufs) b->release();
     if (ctx->h_rows_pinned) cudaFreeHost(ctx->h_rows_pinned);
     for (int i = 0; i < ctx->n_pin; i++) { cudaFreeHost(ctx->pin[i]); cudaEventDestroy(ctx->pin_ev[i]); }
@@ -613,6 +619,118 @@ int mkp_fetch_rows(mkp_ctx* ctx, const mkp_row** rows, size_t* n_rows) {
     }
     *rows = ctx->h_rows_pinned;
     *n_rows = ctx->n_rows;
+    return 0;
+}
+
+// decode (k_parse, k_resolve: the pileup's), rank of the + strand motif positions, k_hemi_count, k_hemi_rows. The counter slots
+// are sized from the chunk's state table (read back after the decode), the rows from the count pass.
+int mkp_hemi_resident(mkp_ctx* ctx, const uint32_t* interval_starts, uint32_t n_intervals, int32_t partner_offset, mkp_stats* stats) {
+    if (!ctx) return -1;
+    if (!ctx->have_params) return fail(ctx, "mkp_set_params was not called");
+    if (ctx->ce <= ctx->cs) return fail(ctx, "no resident chunk");
+    if (!ctx->have_focus) return fail(ctx, "pileup-hemi needs a chunk with motif positions (focus_pos)");
+    if (!interval_starts || n_intervals == 0) return fail(ctx, "pileup-hemi needs the chunk's interval starts");
+    for (uint32_t i = 1; i < n_intervals; i++) if (interval_starts[i] < interval_starts[i - 1]) return fail(ctx, "interval starts must ascend");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    ChunkDev C;
+    const int grid = decode_grid(ctx, ctx->n_reads);
+    if (int rc = prepare_decode(ctx, &C, grid)) return rc;
+    const uint32_t n_words = ctx->n_words;
+    const uint32_t n_blk = (n_words + 1023) / 1024;
+    CK(ctx->d_block_sums.ensure((size_t)n_blk * 4 + 4));
+    CK(ctx->d_row_counts.ensure((size_t)n_words * 4 + 4));
+    CK(ctx->d_row_prefix.ensure((size_t)n_words * 4 + 4));
+    CK(ctx->d_iv_start.ensure((size_t)n_intervals * 4));
+    CK(ctx->d_hemi_hot.ensure((size_t)n_words * 4 + 4));
+    CK(ctx->d_hemi_prefix.ensure((size_t)n_words * 4 + 4));
+    C.hot = ctx->d_hemi_hot.as<uint32_t>();
+    uint32_t* const focus = ctx->d_focus_pos.as<uint32_t>();
+    uint32_t* const focus_prefix = ctx->d_hemi_prefix.as<uint32_t>();
+
+    // events: 0 start | 1 after parse | 2 after resolve | 3 after rank | 4 before counts | 6 after counts | 7 after row count+scan
+    //         | 8 before emit | 9 end
+    CK(cudaEventRecord(ctx->ev[0], st));
+    CK(cudaMemcpyAsync(ctx->d_iv_start.p, interval_starts, (size_t)n_intervals * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(C.hot, 0, (size_t)n_words * 4, st));
+    CK(cudaMemsetAsync(ctx->d_small.p, 0xff, 32 * 8, st));
+    CK(cudaMemsetAsync(ctx->d_small.as<uint8_t>() + 32 * 8, 0, SMALL_BYTES - 32 * 8, st));
+    C.mode = MODE_PILEUP;
+    ctx->launches += 1; if (ctx->n_reads) k_parse<<<grid, 128, 0, st>>>(C);
+    CK(cudaEventRecord(ctx->ev[1], st));
+    ctx->launches += 2; if (ctx->n_reads) { k_resolve<MODE_PILEUP, true><<<grid, 128, 0, st>>>(C); k_resolve<MODE_PILEUP, false><<<grid, 128, 0, st>>>(C); }
+    CK(cudaEventRecord(ctx->ev[2], st));
+    // counter slot of every + strand motif position: its rank in focus_pos (k_block_popc without focus bitmaps only reads it)
+    uint32_t* u = (uint32_t*)(ctx->d_small.as<uint8_t>() + 34 * 8);   // n_states, err, n_hot, n_rows
+    ctx->launches += 1; k_block_popc<<<n_blk, 1024, 0, st>>>(focus, n_words, ctx->d_block_sums.as<uint32_t>(), nullptr, nullptr);
+    ctx->launches += 1; k_scan_blocks<<<1, 1024, 0, st>>>(ctx->d_block_sums.as<uint32_t>(), n_blk, u + 2);
+    ctx->launches += 1; k_word_prefix<<<n_blk, 1024, 0, st>>>(focus, n_words, ctx->d_block_sums.as<uint32_t>(), focus_prefix);
+    CK(cudaEventRecord(ctx->ev[3], st));
+    uint32_t h_small[4];
+    unsigned long long h_calls = 0;
+    CK(cudaMemcpyAsync(h_small, u, 16, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&h_calls, C.total_calls, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    const uint32_t n_states = h_small[0], derr = h_small[1], n_hot = h_small[2];
+    if (derr) {
+        if (stats) { memset(stats, 0, sizeof *stats); stats->device_error = derr; }
+        return fail(ctx, "device decode error: " + derr_text(derr), -10);
+    }
+    const uint32_t n_sides = n_states + 1;
+    const uint32_t stride = 1 + 4 * hemi_base_words(n_sides);
+    CK(ctx->d_slots.ensure(std::max<size_t>(1, n_hot) * stride * 4));
+    CK(cudaMemsetAsync(ctx->d_slots.p, 0, (size_t)n_hot * stride * 4, st));
+    HemiDev D;
+    D.hdrs = C.hdrs; D.heap = C.heap; D.meta = C.meta; D.calls = C.calls; D.n_reads = C.n_reads; D.cs = C.cs; D.ce = C.ce;
+    D.focus = focus; D.focus_prefix = focus_prefix;
+    D.iv_start = ctx->d_iv_start.as<uint32_t>(); D.n_iv = n_intervals;
+    D.partner = partner_offset;
+    D.slots = ctx->d_slots.as<uint32_t>(); D.stride = stride; D.n_sides = n_sides;
+    D.scr_cq = C.scr_cq; D.scr_cr = C.scr_cr; D.scr_stride = ctx->max_ncigar + 4;     // prepare_decode sized them for `grid` blocks of 4 warps
+    D.work = u + 6;
+    CK(cudaEventRecord(ctx->ev[4], st));
+    ctx->launches += 1; if (ctx->n_reads && n_hot) k_hemi_count<<<grid, 128, 0, st>>>(D);
+    CK(cudaEventRecord(ctx->ev[6], st));
+    HemiRowDev R;
+    R.focus = focus; R.focus_prefix = focus_prefix; R.n_words = n_words; R.cs = C.cs;
+    R.slots = D.slots; R.stride = stride; R.n_sides = n_sides; R.states = C.states; R.combine = ctx->params.numeric_mode == 1;
+    R.row_counts = ctx->d_row_counts.as<uint32_t>(); R.row_prefix = ctx->d_row_prefix.as<uint32_t>(); R.rows = nullptr;
+    const int rg = (n_words + 255) / 256;
+    ctx->launches += 1; k_hemi_rows<false><<<rg, 256, 0, st>>>(R);
+    ctx->launches += 1; k_block_sum<<<n_blk, 1024, 0, st>>>(R.row_counts, n_words, ctx->d_block_sums.as<uint32_t>());
+    ctx->launches += 1; k_scan_blocks<<<1, 1024, 0, st>>>(ctx->d_block_sums.as<uint32_t>(), n_blk, u + 3);
+    ctx->launches += 1; k_value_prefix<<<n_blk, 1024, 0, st>>>(R.row_counts, n_words, ctx->d_block_sums.as<uint32_t>(), ctx->d_row_prefix.as<uint32_t>());
+    CK(cudaEventRecord(ctx->ev[7], st));
+    uint32_t n_rows = 0;
+    CK(cudaMemcpyAsync(&n_rows, u + 3, 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    CK(ctx->d_hemi_rows.ensure(std::max<size_t>(1, n_rows) * sizeof(mkp_hemi_row)));
+    R.rows = ctx->d_hemi_rows.as<mkp_hemi_row>();
+    CK(cudaEventRecord(ctx->ev[8], st));
+    ctx->launches += 1; if (n_rows) k_hemi_rows<true><<<rg, 256, 0, st>>>(R);
+    CK(cudaEventRecord(ctx->ev[9], st));
+    CK(cudaStreamSynchronize(st));
+    CK(cudaGetLastError());
+    ctx->n_hemi_rows = n_rows;
+    if (stats) {
+        memset(stats, 0, sizeof *stats);
+        stats->n_rows = n_rows; stats->n_hot = n_hot; stats->n_calls = h_calls; stats->n_states = n_states;
+        // kernel_ms: 0 parse, 1 resolve, 2 rank, 4 counters (k_hemi_count), 5 rows (count+scan+emit), 6 host syncs/allocs, 7 total
+        auto el = [&](int a, int b) { float ms = 0; cudaEventElapsedTime(&ms, ctx->ev[a], ctx->ev[b]); return ms; };
+        stats->kernel_ms[0] = el(0, 1); stats->kernel_ms[1] = el(1, 2); stats->kernel_ms[2] = el(2, 3);
+        stats->kernel_ms[4] = el(4, 6); stats->kernel_ms[5] = el(6, 7) + el(8, 9);
+        stats->kernel_ms[6] = el(3, 4) + el(7, 8); stats->kernel_ms[7] = el(0, 9);
+    }
+    return 0;
+}
+
+int mkp_fetch_hemi_rows(mkp_ctx* ctx, const mkp_hemi_row** rows, size_t* n_rows) {
+    if (!ctx || !rows || !n_rows) return -1;
+    CK(cudaSetDevice(ctx->device));
+    ctx->h_hemi_rows.resize(std::max<size_t>(1, ctx->n_hemi_rows));
+    if (ctx->n_hemi_rows) CK(cudaMemcpy(ctx->h_hemi_rows.data(), ctx->d_hemi_rows.p, ctx->n_hemi_rows * sizeof(mkp_hemi_row), cudaMemcpyDeviceToHost));
+    *rows = ctx->h_hemi_rows.data();
+    *n_rows = ctx->n_hemi_rows;
     return 0;
 }
 

@@ -11,6 +11,8 @@
 //   k_count_bases warp per read: walks CIGAR + SEQ with bit-parallel window tests against the hot
 //                 bitmap; base / delete counters and observed-code masks (src/pileup/mod.rs:831-874)
 //   k_rows_*      per slot: FeatureVector::decode (src/pileup/mod.rs:283-445) -> mkp_row
+//   k_hemi_count, k_hemi_rows   `pileup-hemi` over the same decode: duplex pattern counters per + strand motif position and
+//                 DuplexFeatureVector::decode -> mkp_hemi_row (src/pileup/duplex.rs)
 // Integer/indexing work: no tensor cores; the bound is HBM bandwidth.
 #pragma once
 #include <cuda_runtime.h>
@@ -1886,6 +1888,279 @@ __global__ void k_value_prefix(const uint32_t* __restrict__ v, uint32_t n, const
     if (threadIdx.x < 32) { uint32_t t = s_w[threadIdx.x]; uint32_t ti = warp_incl_scan(t); s_w[threadIdx.x] = ti - t; }
     __syncthreads();
     if (i < n) prefix[i] = block_sums[blockIdx.x] + s_w[threadIdx.x >> 5] + inc - x;
+}
+
+// ---- pileup-hemi (src/pileup/duplex.rs, src/read_cache.rs:368-468) ---------------------------------------------------------
+// Per + strand motif position p (the chunk's focus_pos bitmap) and admitted read: a deletion counts n_delete; an ACGT SEQ base
+// pairs the read's call on the + strand at p with its call on the - strand at p + partner, looked up in the table of the
+// complementary base. Counter slot of a position = its rank in focus_pos; layout (u32): [0] n_delete, then per primary base
+// (SEQ base at p) [filtered, nocall, pattern[pos side][neg side]], side 0 = canonical, 1 + id = mod state id.
+struct HemiDev {
+    const mkp_read_hdr* hdrs;
+    const uint8_t* heap;
+    const ReadMeta* meta;
+    const uint2* calls;
+    uint32_t n_reads, cs, ce;              // call window (the focus bits lie inside it)
+    const uint32_t* focus; const uint32_t* focus_prefix;
+    const uint32_t* iv_start; uint32_t n_iv;   // starts of the chunk's intervals, non-decreasing
+    int32_t partner;                       // reverse offset - forward offset of the motif
+    uint32_t* slots;
+    uint32_t stride, n_sides;              // n_sides = n_states + 1
+    uint32_t* scr_cq; uint32_t* scr_cr; uint32_t scr_stride;   // per-warp CIGAR prefix (query / reference start of every op)
+    uint32_t* work;
+};
+
+__host__ __device__ __forceinline__ uint32_t hemi_base_words(uint32_t n_sides) { return 2u + n_sides * n_sides; }
+
+// warp per read. The read's call records are one monotone run per MM list (ascending positions on a forward read, descending
+// on a reverse one): a lookup is one binary search per run.
+__global__ void __launch_bounds__(128) k_hemi_count(HemiDev D) {
+    __shared__ uint32_t s_seg[4][MAX_LISTS + 2];
+    const uint32_t lane = lane_id();
+    const uint32_t wib = threadIdx.x >> 5;
+    const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    uint32_t* const cq = D.scr_cq + (size_t)gw * D.scr_stride;
+    uint32_t* const cr = D.scr_cr + (size_t)gw * D.scr_stride;
+    const uint32_t bw = hemi_base_words(D.n_sides);
+    for (;;) {
+        uint32_t ri = 0;
+        if (lane == 0) ri = atomicAdd(D.work, 1u);
+        ri = __shfl_sync(FULL, ri, 0);
+        if (ri >= D.n_reads) break;
+        const ReadMeta m = D.meta[ri];
+        if (!(m.flags & 1)) continue;
+        const mkp_read_hdr h = D.hdrs[ri];
+        if ((uint32_t)m.ref_end <= D.cs || (uint32_t)h.ref_start >= D.ce) continue;
+        const uint32_t lo_r = (uint32_t)h.ref_start > D.cs ? (uint32_t)h.ref_start : D.cs;
+        const uint32_t hi_r = (uint32_t)m.ref_end < D.ce ? (uint32_t)m.ref_end : D.ce;
+        const uint32_t a = (h.flags & 0x10) ? 1u : 0u;
+        const bool failed = !(m.flags & 2);           // skip_set: no usable mod info
+        const uint32_t* cig = (const uint32_t*)(D.heap + h.off);
+        const uint8_t* seq = D.heap + h.off + 4ull * h.n_cigar;
+        const uint32_t nc = h.n_cigar;
+        __syncwarp();
+        {
+            uint32_t qc = 0, rc = (uint32_t)h.ref_start;
+            for (uint32_t b0 = 0; b0 < nc; b0 += 32) {
+                const uint32_t i = b0 + lane;
+                const uint32_t c = i < nc ? cig[i] : 0u, op = c & 15, len = c >> 4;
+                const uint32_t ql = (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) ? len : 0;
+                const uint32_t rl = (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) ? len : 0;
+                const uint32_t qi = warp_incl_scan(ql), rr = warp_incl_scan(rl);
+                if (i < nc) { cq[i] = qc + qi - ql; cr[i] = rc + rr - rl; }
+                qc += __shfl_sync(FULL, qi, 31);
+                rc += __shfl_sync(FULL, rr, 31);
+            }
+        }
+        // monotone runs of the records: s_seg[0..n_seg] are their boundaries
+        const uint2* rcalls = D.calls + m.entry_off;
+        const uint32_t n = failed ? 0u : m.n_calls;
+        uint32_t n_seg = 1;
+        if (lane == 0) s_seg[wib][0] = 0;
+        for (uint32_t k0 = 1; k0 < n; k0 += 32) {
+            const uint32_t k = k0 + lane;
+            bool brk = false;
+            if (k < n) { const uint32_t x1 = rcalls[k].x, x0 = rcalls[k - 1].x; brk = a ? x1 > x0 : x1 < x0; }
+            const uint32_t bm = __ballot_sync(FULL, brk);
+            if (brk) { const uint32_t at = n_seg + __popc(bm & ((1u << lane) - 1u)); if (at <= MAX_LISTS) s_seg[wib][at] = k; }
+            n_seg += __popc(bm);
+        }
+        if (n_seg > MAX_LISTS) n_seg = MAX_LISTS;     // (one run per MM list, at most MAX_LISTS lists)
+        if (lane == 0) s_seg[wib][n_seg] = n;
+        __syncwarp();
+        // the op under reference position r: 0 none (outside, reference skip), 1 aligned base at query *q, 2 deletion
+        auto op_at = [&](uint32_t r, uint32_t* q) -> uint32_t {
+            if (nc == 0 || r < cr[0]) return 0;
+            uint32_t lo = 0, hi = nc;
+            while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (cr[mid] <= r) lo = mid; else hi = mid; }
+            const uint32_t c = cig[lo], op = c & 15, len = c >> 4;
+            if (r >= cr[lo] + len) return 0;
+            if (op == 0 || op == 7 || op == 8) { *q = cq[lo] + (r - cr[lo]); return *q < h.l_seq ? 1u : 0u; }
+            return op == 2 ? 2u : 0u;
+        };
+        // the read's call at r on mod strand st, forward base cb: state + 1 (1 filtered, 2 canonical, 3 + id), 0 = none
+        auto call_at = [&](uint32_t r, uint32_t q, uint32_t st, uint32_t cb) -> uint32_t {
+            for (uint32_t s = 0; s < n_seg; s++) {
+                const uint32_t end = s_seg[wib][s + 1];
+                uint32_t lo = s_seg[wib][s], hi = end;
+                while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; const uint32_t x = rcalls[mid].x; if (a ? x > r : x < r) lo = mid + 1; else hi = mid; }
+                for (uint32_t k = lo; k < end; k++) {
+                    const uint2 c = rcalls[k];
+                    if (c.x != r) break;
+                    if ((c.y & 1u) == st && ((c.y >> 1) & 3u) == cb) return ((c.y >> 3) & 0xffu) + 1u;
+                }
+            }
+            // implicit table: every other occurrence of its base is an inferred-canonical entry, subject to the edge filter
+            const uint32_t imp = (m.imp[st] >> (8 * cb)) & 0xffu;
+            if (!(imp & 0x80u)) return 0;
+            const uint32_t f = a ? h.l_seq - 1u - q : q;
+            if (c_par.edge_on && !(c_par.edge_inv ? (f < c_par.edge_start || f >= h.l_seq - c_par.edge_end) : (f >= c_par.edge_start && f < h.l_seq - c_par.edge_end))) return 0;
+            return (imp & 0x7fu) + 1u;
+        };
+        if (lo_r >= hi_r) continue;
+        const uint32_t w0 = (lo_r - D.cs) >> 5, w1 = (hi_r - 1 - D.cs) >> 5;
+        auto word_bits = [&](uint32_t w) {
+            uint32_t bits = D.focus[w];
+            const uint32_t wbase = D.cs + (w << 5);
+            if (lo_r > wbase) bits &= FULL << (lo_r - wbase);
+            if (hi_r < wbase + 32) bits &= (1u << (hi_r - wbase)) - 1u;
+            return bits;
+        };
+        auto slot = [&](uint32_t w, uint32_t bit) { return D.slots + (size_t)(D.focus_prefix[w] + __popc(D.focus[w] & ((1u << bit) - 1u))) * D.stride; };
+        if (!failed) {
+            for (uint32_t w = w0 + lane; w <= w1; w += 32) {
+                uint32_t bits = word_bits(w);
+                while (bits) {
+                    const uint32_t bit = __ffs(bits) - 1;
+                    bits &= bits - 1;
+                    const uint32_t r = D.cs + (w << 5) + bit;
+                    uint32_t q = 0;
+                    const uint32_t kind = op_at(r, &q);
+                    if (!kind) continue;
+                    uint32_t* S = slot(w, bit);
+                    if (kind == 2) { atomicAdd(&S[0], 1u); continue; }
+                    const int nb = nib_to_base(seq_nibble(seq, q));
+                    if (nb > 3) continue;
+                    uint32_t* B = S + 1 + (uint32_t)nb * bw;
+                    const uint32_t cb = a ? 3u - (uint32_t)nb : (uint32_t)nb;
+                    const uint32_t vp = call_at(r, q, a, cb);
+                    uint32_t vn = 0;
+                    const int64_t rn = (int64_t)r + D.partner;
+                    if (vp && rn >= 0) {
+                        uint32_t qn = 0;
+                        if (op_at((uint32_t)rn, &qn) == 1 && nib_to_base(seq_nibble(seq, qn)) == 3 - nb) vn = call_at((uint32_t)rn, qn, 1u - a, 3u - cb);
+                    }
+                    if (!vp || !vn) atomicAdd(&B[1], 1u);
+                    else if (vp == 1 || vn == 1) atomicAdd(&B[0], 1u);
+                    else atomicAdd(&B[2 + (vp - 2) * D.n_sides + (vn - 2)], 1u);
+                }
+            }
+        } else {
+            // the read cache checks its skip set before the first decode: a read without usable mod info is one NoCall, at its
+            // first motif position with an ACGT base in each interval (the reference's cache lives for one interval). Its
+            // deletions count like any read's.
+            uint32_t iv_done = 0xffffffffu;
+            for (uint32_t wt = w0; wt <= w1; wt += 32) {
+                const uint32_t w = wt + lane;
+                uint32_t ok = 0;
+                if (w <= w1) {
+                    uint32_t bits = word_bits(w);
+                    while (bits) {
+                        const uint32_t bit = __ffs(bits) - 1;
+                        bits &= bits - 1;
+                        uint32_t q = 0;
+                        const uint32_t kind = op_at(D.cs + (w << 5) + bit, &q);
+                        if (kind == 2) atomicAdd(&slot(w, bit)[0], 1u);
+                        else if (kind == 1 && nib_to_base(seq_nibble(seq, q)) <= 3) ok |= 1u << bit;
+                    }
+                }
+                uint32_t lanes = __ballot_sync(FULL, ok != 0);
+                while (lanes) {
+                    const uint32_t src = __ffs(lanes) - 1;
+                    lanes &= lanes - 1;
+                    uint32_t bits = __shfl_sync(FULL, ok, src);
+                    while (bits) {
+                        const uint32_t bit = __ffs(bits) - 1;
+                        bits &= bits - 1;
+                        const uint32_t r = D.cs + ((wt + src) << 5) + bit;
+                        uint32_t lo = 0, hi = D.n_iv;          // interval of r: the last start <= r
+                        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (D.iv_start[mid] <= r) lo = mid; else hi = mid; }
+                        if (lo == iv_done) continue;
+                        iv_done = lo;
+                        if (lane == 0) {
+                            uint32_t q = 0;
+                            op_at(r, &q);
+                            const uint32_t nb = (uint32_t)nib_to_base(seq_nibble(seq, q));
+                            atomicAdd(&slot(wt + src, bit)[1 + nb * bw + 1], 1u);
+                        }
+                    }
+                }
+            }
+        }
+    }
+}
+
+struct HemiRowDev {
+    const uint32_t* focus; const uint32_t* focus_prefix;
+    uint32_t n_words, cs;
+    const uint32_t* slots;
+    uint32_t stride, n_sides;
+    const unsigned long long* states;   // registry: (pb << 32 | code)
+    uint32_t combine;                   // --combine-mods: mod codes -> the base's any-mod code (DuplexModCall::into_combined)
+    uint32_t* row_counts;               // per focus word
+    const uint32_t* row_prefix;
+    mkp_hemi_row* rows;
+};
+
+// DuplexFeatureVector::decode (src/pileup/duplex.rs:121-204) of one slot, rows by base then pattern. out == nullptr => count only
+__device__ uint32_t hemi_slot_rows(const HemiRowDev& R, const uint32_t* S, uint32_t pos, mkp_hemi_row* out) {
+    const uint32_t ns = R.n_sides, bw = hemi_base_words(ns);
+    uint32_t tot[4], all = 0;
+    for (uint32_t pb = 0; pb < 4; pb++) {
+        const uint32_t* B = S + 1 + pb * bw;
+        uint32_t t = 0;
+        for (uint32_t k = 0; k < ns * ns; k++) t += B[2 + k];
+        tot[pb] = t;
+        all += t;
+    }
+    uint32_t n = 0;
+    for (uint32_t pb = 0; pb < 4; pb++) {
+        if (!tot[pb]) continue;                     // a base without a pattern has no row
+        const uint32_t* B = S + 1 + pb * bw;
+        mkp_hemi_row r;
+        r.pos = pos; r.primary_base = pb;
+        r.n_canonical = B[2]; r.n_delete = S[0]; r.n_fail = B[0]; r.n_nocall = B[1]; r.n_diff = all - tot[pb];
+        if (R.combine) {
+            uint32_t c[2][2] = {{0, 0}, {0, 0}};
+            for (uint32_t sp = 0; sp < ns; sp++) for (uint32_t sn = 0; sn < ns; sn++) c[sp > 0][sn > 0] += B[2 + sp * ns + sn];
+            const uint32_t any = (uint32_t)("ACGT"[pb]);
+            for (uint32_t i = 0; i < 2; i++) for (uint32_t j = 0; j < 2; j++) {
+                if (!c[i][j]) continue;
+                r.code_pos = i ? any : MKP_HEMI_CANONICAL; r.code_neg = j ? any : MKP_HEMI_CANONICAL;
+                r.count = c[i][j]; r.n_other_pattern = tot[pb] - c[i][j];
+                if (out) out[n] = r;
+                n++;
+            }
+            continue;
+        }
+        const uint32_t row0 = n;
+        for (uint32_t sp = 0; sp < ns; sp++) for (uint32_t sn = 0; sn < ns; sn++) {
+            const uint32_t cnt = B[2 + sp * ns + sn];
+            if (!cnt) continue;
+            r.code_pos = sp ? (uint32_t)R.states[sp - 1] : MKP_HEMI_CANONICAL;
+            r.code_neg = sn ? (uint32_t)R.states[sn - 1] : MKP_HEMI_CANONICAL;
+            r.count = cnt; r.n_other_pattern = tot[pb] - cnt;
+            if (out) out[n] = r;
+            n++;
+        }
+        // insertion sort by pattern (derived Ord: Canonical < Code(char) < ChEbi, first element then second == u32 order here)
+        if (out) for (uint32_t i = row0 + 1; i < n; i++) {
+            const mkp_hemi_row key = out[i];
+            uint32_t j = i;
+            while (j > row0 && (out[j - 1].code_pos > key.code_pos || (out[j - 1].code_pos == key.code_pos && out[j - 1].code_neg > key.code_neg))) { out[j] = out[j - 1]; j--; }
+            out[j] = key;
+        }
+    }
+    return n;
+}
+
+// thread per focus word: count pass (EMIT = false), then the emit pass at the scanned offsets
+template <bool EMIT>
+__global__ void __launch_bounds__(256) k_hemi_rows(HemiRowDev R) {
+    const uint32_t w = blockIdx.x * blockDim.x + threadIdx.x;
+    if (w >= R.n_words) return;
+    uint32_t bits = R.focus[w];
+    if (!bits) { if (!EMIT) R.row_counts[w] = 0; return; }
+    uint32_t slot = R.focus_prefix[w];
+    mkp_hemi_row* out = EMIT ? R.rows + R.row_prefix[w] : nullptr;
+    uint32_t n = 0;
+    while (bits) {
+        const uint32_t bit = __ffs(bits) - 1;
+        bits &= bits - 1;
+        n += hemi_slot_rows(R, R.slots + (size_t)slot * R.stride, R.cs + (w << 5) + bit, EMIT ? out + n : nullptr);
+        slot++;
+    }
+    if (!EMIT) R.row_counts[w] = n;
 }
 
 // ---- processing order: reads by descending length class (32 classes by the position of the top bit of l_seq); a counting sort,

@@ -7,6 +7,9 @@
 //                [--mean-len 12000] [--level 1] [--threads 8] [--combined-hm] [--implicit] [--odd-records] [--partition-tags [--long-rg]]
 //                [--start-grid G]  (read starts snapped to multiples of G: stacks of reads sharing a start, for --max-depth)
 //                [--region-only START-END]   (only reads overlapping the window; reference still full length)
+//                [--duplex]  (duplex basecalls: G-h?/G-m? lists for the opposite strand's C of every CpG beside the C+ lists, T-a?
+//                             beside A+a?; 3% of
+//                             the reads without MM/ML, 3% with an MN tag that does not match the sequence length)
 // Writes PREFIX.fa, PREFIX.fa.fai, PREFIX.bam, PREFIX.bam.bai and prints a JSON summary (exact algorithmic bytes,
 // read-bases, reads) on stdout.
 #include <zlib.h>
@@ -46,7 +49,7 @@ struct Opts {
     std::string mods = "m";
     double mean_len = 12000, sigma = 0.6;
     int level = 1, threads = 8;
-    bool combined_hm = false, implicit = false, odd = false;
+    bool combined_hm = false, implicit = false, odd = false, duplex = false;
     bool ptags = false;    // --partition-tags: RG:Z (A/B/C or absent), HP (C or i, or absent), XF:f on some reads
     bool long_rg = false;  // --long-rg: the RG values are long run ids (ONT style, ~80 characters) ending in A/B/C
     int64_t win_start = -1, win_end = -1;
@@ -145,6 +148,8 @@ static void make_read(const Opts& o, const Contig& c, int32_t tid, uint32_t star
         else if (u < 0.06) with_tags = false;
         else if (u < 0.10) mn_tag = true;
     }
+    bool mn_bad = false;
+    if (o.duplex) { const double u = rng.uni(); if (u < 0.03) with_tags = false; else if (u < 0.06) mn_bad = true; }
     const char mode = o.implicit ? '.' : '?';
     if (with_tags) {
         const bool want_h = o.mods.find('h') != std::string::npos, want_m = o.mods.find('m') != std::string::npos, want_a = o.mods.find('a') != std::string::npos;
@@ -184,6 +189,37 @@ static void make_read(const Opts& o, const Contig& c, int32_t tid, uint32_t star
                 else { emit(std::string("C+h") + mode, &qh, nullptr); emit(std::string("C+m") + mode, &qm, nullptr); }
             } else if (want_m) emit(std::string("C+m") + mode, &qm, nullptr);
             else emit(std::string("C+h") + mode, &qh, nullptr);
+            if (o.duplex) {
+                // the other strand of each CpG, called on the read's G (mod strand '-'): independent draws at the site's level
+                std::vector<uint32_t> gd;
+                std::vector<uint8_t> gh, gm;
+                uint32_t gskip = 0;
+                for (uint32_t f = 0; f < L; f++) {
+                    if (fwd(f) != 'G') continue;
+                    if (!(f > 0 && fwd(f - 1) == 'C')) { gskip++; continue; }
+                    gd.push_back(gskip);
+                    gskip = 0;
+                    const int64_t rp = fwd_ref(f);
+                    double level = 0.5;
+                    if (rp >= 1) { const uint32_t cpos = rev ? (uint32_t)rp : (uint32_t)rp - 1; if (cpos < c.len) level = c.meth[cpos] / 255.0; }
+                    const bool confident = rng.uni() < 0.8;
+                    const bool is_mod = rng.uni() < level;
+                    const bool is_h = want_h && is_mod && rng.uni() < 0.15;
+                    uint32_t qa, qb;
+                    if (confident) { qa = 230 + rng.below(26); qb = rng.below(256 - qa); } else { qa = rng.below(256); qb = rng.below(256 - qa); }
+                    if (!is_mod) { uint32_t lo = rng.below(26); qa = confident ? lo : qa; qb = confident ? rng.below(26) : qb; if (qa + qb > 255) qb = 255 - qa; }
+                    if (want_h && want_m) { if (is_h) { gh.push_back((uint8_t)qa); gm.push_back((uint8_t)qb); } else { gm.push_back((uint8_t)qa); gh.push_back((uint8_t)qb); } }
+                    else if (want_m) gm.push_back((uint8_t)qa);
+                    else gh.push_back((uint8_t)qa);
+                }
+                deltas.swap(gd);
+                if (want_h && want_m) {
+                    if (o.combined_hm) emit(std::string("G-hm") + mode, &gh, &gm);
+                    else { emit(std::string("G-h") + mode, &gh, nullptr); emit(std::string("G-m") + mode, &gm, nullptr); }
+                } else if (want_m) emit(std::string("G-m") + mode, &gm, nullptr);
+                else emit(std::string("G-h") + mode, &gh, nullptr);
+                deltas.swap(gd);
+            }
         }
         if (want_a) {
             mm += std::string("A+a") + mode;
@@ -198,6 +234,20 @@ static void make_read(const Opts& o, const Contig& c, int32_t tid, uint32_t star
                 ml.push_back(rng.uni() < 0.03 ? (uint8_t)(200 + rng.below(56)) : (uint8_t)rng.below(40));
             }
             mm += ';';
+            if (o.duplex) {
+                // the other strand's A, called on the read's T
+                mm += std::string("T-a") + mode;
+                skipped = 0;
+                for (uint32_t f = 0; f < L; f++) {
+                    if (fwd(f) != 'T') continue;
+                    if (rng.uni() < 0.02) { skipped++; continue; }
+                    int n = snprintf(buf, sizeof buf, ",%u", skipped);
+                    mm.append(buf, n);
+                    skipped = 0;
+                    ml.push_back(rng.uni() < 0.03 ? (uint8_t)(200 + rng.below(56)) : (uint8_t)rng.below(40));
+                }
+                mm += ';';
+            }
         }
     }
     if (!emit_read) return;
@@ -218,7 +268,7 @@ static void make_read(const Opts& o, const Contig& c, int32_t tid, uint32_t star
     for (uint32_t i = 0; i < L; i += 2) v.push_back((uint8_t)(nib(seq[i]) << 4 | (i + 1 < L ? nib(seq[i + 1]) : 0)));
     v.insert(v.end(), L, 0xff);
     if (with_tags) {
-        if (mn_tag) { v.push_back('M'); v.push_back('N'); v.push_back('i'); put<int32_t>(v, (int32_t)L); }
+        if (mn_tag || mn_bad) { v.push_back('M'); v.push_back('N'); v.push_back('i'); put<int32_t>(v, (int32_t)L + (mn_bad ? 1 : 0)); }
         v.push_back('M'); v.push_back('M'); v.push_back('Z'); v.insert(v.end(), mm.begin(), mm.end()); v.push_back(0);
         v.push_back('M'); v.push_back('L'); v.push_back('B'); v.push_back('C'); put<uint32_t>(v, (uint32_t)ml.size()); v.insert(v.end(), ml.begin(), ml.end());
     }
@@ -256,6 +306,7 @@ int main(int argc, char** argv) {
         else if (a == "--combined-hm") o.combined_hm = true;
         else if (a == "--implicit") o.implicit = true;
         else if (a == "--odd-records") o.odd = true;
+        else if (a == "--duplex") o.duplex = true;
         else if (a == "--partition-tags") o.ptags = true;
         else if (a == "--long-rg") o.long_rg = true;
         else if (a == "--start-grid") o.start_grid = (uint32_t)std::stoul(val());
