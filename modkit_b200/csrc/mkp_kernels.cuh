@@ -382,8 +382,11 @@ __device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t* P, uint32_t 
 #ifndef MKP_MINB_RESOLVE
 #define MKP_MINB_RESOLVE 7
 #endif
+// k_count_bases: 5 blocks of 256 threads = 48 registers, which leaves 12 bytes of spills. At 8 blocks (32 registers) its hot loop
+// spilled 128 / 152 bytes and the kernel took 1.41x as long on an H100 (profiles/README.md); 4 blocks (64 registers, no spills) is
+// slower than 5: the walk is latency bound and wants the warps
 #ifndef MKP_MINB_BASES
-#define MKP_MINB_BASES 8
+#define MKP_MINB_BASES 5
 #endif
 __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
     __shared__ ListTab s_tab[4];
