@@ -28,21 +28,24 @@ inline int32_t rdi32(const uint8_t* p) { int32_t v; memcpy(&v, p, 4); return v; 
 struct BamRecord {
     const uint8_t* data = nullptr;  // points at refID (after block_size)
     uint32_t size = 0;              // block_size
+    const uint8_t* cg = nullptr;    // the CG:B,I array when the core CIGAR is its placeholder (attach_long_cigar)
+    uint32_t n_cg = 0;
     int32_t tid() const { return rdi32(data); }
     int32_t pos() const { return rdi32(data + 4); }
     uint8_t l_name() const { return data[8]; }
-    uint16_t n_cigar() const { return rd16(data + 12); }
+    uint16_t n_cigar_core() const { return rd16(data + 12); }   // the ops stored in the record's core (its layout)
+    uint32_t n_cigar() const { return cg ? n_cg : n_cigar_core(); }
     uint16_t flag() const { return rd16(data + 14); }
     int32_t l_seq() const { return rdi32(data + 16); }
     const char* name() const { return (const char*)(data + 32); }
     const uint8_t* cigar() const { return data + 32 + l_name(); }
-    const uint8_t* seq() const { return cigar() + 4 * (size_t)n_cigar(); }
+    const uint8_t* seq() const { return cigar() + 4 * (size_t)n_cigar_core(); }
     const uint8_t* qual() const { return seq() + (l_seq() + 1) / 2; }
     const uint8_t* aux() const { return qual() + l_seq(); }
     const uint8_t* end() const { return data + size; }
     bool is_reverse() const { return flag() & 0x10; }
     bool is_unmapped() const { return flag() & 0x4; }
-    uint32_t cigar_op(int i) const { return rd32(cigar() + 4 * i); }
+    uint32_t cigar_op(int i) const { return rd32((cg ? cg : cigar()) + 4 * (size_t)i); }
     // reference length consumed (M,D,N,=,X)
     int64_t rlen() const {
         int64_t r = 0;
@@ -111,6 +114,19 @@ inline bool find_aux(const BamRecord& r, const char tag[2], AuxField* out) {
         p += sz;
     }
     return false;
+}
+
+// Long CIGARs (more than 65535 ops, SAMv1 4.2.2): the core holds the placeholder `<l_seq>S <ref_len>N` and the real CIGAR is
+// the CG:B,I array. htslib swaps the array in when it reads the record. The rule applied here is the product's packer's: two
+// core ops, the first a soft clip of the whole query, and a CG tag of type B,I (DESIGN 7).
+inline void attach_long_cigar(BamRecord* r) {
+    r->cg = nullptr;
+    r->n_cg = 0;
+    if (r->n_cigar_core() != 2) return;
+    const uint32_t c0 = rd32(r->cigar());
+    if ((c0 & 0xf) != 4 || (int64_t)(c0 >> 4) != (int64_t)r->l_seq()) return;
+    AuxField f;
+    if (find_aux(*r, "CG", &f) && f.type == 'B' && f.subtype == 'I') { r->cg = f.p; r->n_cg = f.n; }
 }
 
 struct BamFile {
@@ -218,6 +234,7 @@ struct BamFile {
             BamRecord r;
             r.data = p + 4;
             r.size = bs;
+            attach_long_cigar(&r);
             uint32_t idx = (uint32_t)records.size();
             records.push_back(r);
             int32_t tid = r.tid();

@@ -20,8 +20,16 @@ static void die(const std::string& m) { fprintf(stderr, "> Error! %s\n", m.c_str
 //   decode SEQ MM ML_CSV [ignore_code]  -> one line per table entry: strand base pos inferred code:prob[,code:prob] canonical_prob
 //   call BASE code:p[,code:p] default [B:thr ...] [mod=c:thr ...] -> filtered | canonical P | modified CODE P
 //   percentile Q v0,v1,...
+//   endpos IN.BAM -> one line per record in file order: name pos endpos n_cigar (the CIGAR accessors, CG:B,I applied)
 static int kat_main(int argc, char** argv) {
     std::string cmd = argv[1];
+    if (cmd == "endpos") {
+        if (argc < 3) return 2;
+        BamFile bam;
+        bam.load(argv[2]);
+        for (const BamRecord& r : bam.records) printf("%s %d %lld %u\n", r.name(), r.pos(), (long long)r.endpos(), r.n_cigar());
+        return 0;
+    }
     if (cmd == "decode") {
         if (argc < 5) return 2;
         std::string seq = argv[2], mm = argv[3], mlcsv = argv[4];
@@ -187,7 +195,7 @@ static int sample_main(int argc, char** argv) {
 
 int main(int argc, char** argv) {
     try {
-        if (argc >= 2 && (std::string(argv[1]) == "decode" || std::string(argv[1]) == "call" || std::string(argv[1]) == "percentile")) return kat_main(argc, argv);
+        if (argc >= 2 && (std::string(argv[1]) == "decode" || std::string(argv[1]) == "call" || std::string(argv[1]) == "percentile" || std::string(argv[1]) == "endpos")) return kat_main(argc, argv);
         if (argc >= 2 && (std::string(argv[1]) == "summary" || std::string(argv[1]) == "sample-probs")) return sample_main(argc, argv);
         if (argc < 2 || std::string(argv[1]) != "pileup") die("usage: modkit_oracle pileup [flags] <in.bam> <out.bed>");
         std::vector<std::string> pos;

@@ -1,7 +1,8 @@
 """Tiny pure-Python BGZF/BAM reader + writer for tests and fixture preparation (no pysam/htslib here).
 
-Only what the tests need: iterate records, look at / rewrite aux tags, write a coordinate-sorted BAM
-back out (BGZF members of <= 64 KiB, EOF marker). Not used by the product path.
+Only what the tests need: iterate records, look at / rewrite aux tags, build records of an exact shape (make_record,
+mm_for), write a coordinate-sorted BAM back out (BGZF members of <= 64 KiB, EOF marker) and a FASTA with its .fai.
+Not used by the product path.
 """
 import struct
 import zlib
@@ -214,3 +215,106 @@ def replace_aux(r, mapping):
         else:
             out.append(r[s:e])
     return b"".join(out)
+
+
+CIGAR_OPS = "MIDNSHP=X"
+SEQ_NIB = "=ACMGRSVTWYHKDBN"
+COMPLEMENT = str.maketrans("ACGTRYKMSWBVDHN", "TGCAYRMKSWVBHDN")
+
+
+def revcomp(seq):
+    return seq.translate(COMPLEMENT)[::-1]
+
+
+def cigar_spans(cigar):
+    """(query length, reference length) consumed by a [(op char, len)] CIGAR."""
+    return (sum(n for op, n in cigar if op in "MIS=X"), sum(n for op, n in cigar if op in "MDN=X"))
+
+
+def aux_z(tag, text):
+    return tag.encode() + b"Z" + (text.encode() if isinstance(text, str) else text) + b"\x00"
+
+
+def aux_b(tag, sub, values):
+    fmt = {"c": "b", "C": "B", "s": "h", "S": "H", "i": "i", "I": "I", "f": "f"}[sub]
+    return tag.encode() + b"B" + sub.encode() + struct.pack("<I%d%s" % (len(values), fmt), len(values), *values)
+
+
+def aux_i(tag, value):
+    return tag.encode() + b"i" + struct.pack("<i", value)
+
+
+def make_record(tid, pos, flag, cigar, seq, mm=None, ml=None, aux=(), name="r", long_cigar=False, cg_at="last", mapq=60):
+    """Raw bytes (without block_size) of one BAM record.
+
+    cigar: [(op char, len)]; seq: bases, IUPAC letters allowed, "" for SEQ *; qualities are 0xff. mm / ml: the MM text and
+    the ML probabilities (ints 0-255) in read orientation, or None to leave the tags out; aux: further encoded fields
+    (aux_z, aux_i, aux_b), written after MM/ML. long_cigar=True stores the CIGAR in CG:B,I with the SAMv1 4.2.2 placeholder
+    `<l_seq>S <ref_len>N` in the core; cg_at puts the CG field "first", "middle" (between MM and ML) or "last"."""
+    ops = [(CIGAR_OPS.index(op), n) for op, n in cigar]
+    words = [n << 4 | op for op, n in ops]
+    _, rlen = cigar_spans(cigar)
+    core = [len(seq) << 4 | 4, rlen << 4 | 3] if long_cigar else words
+    end = pos + (rlen if rlen and not flag & 4 else 1)
+    nb = name.encode() + b"\x00"
+    packed = bytearray((len(seq) + 1) // 2)
+    for i, c in enumerate(seq):
+        packed[i >> 1] |= SEQ_NIB.index(c.upper()) << (0 if i & 1 else 4)
+    fields = []
+    if mm is not None:
+        fields.append(aux_z("MM", mm))
+    if ml is not None:
+        fields.append(aux_b("ML", "C", list(ml)))
+    if long_cigar:
+        cg = aux_b("CG", "I", words)
+        fields.insert({"first": 0, "middle": 1 if mm is not None else 0, "last": len(fields)}[cg_at], cg)
+    fields += list(aux)
+    head = struct.pack("<iiBBHHHiiii", tid, pos, len(nb), mapq, reg2bin(pos, end), len(core), flag, len(seq), -1, -1, 0)
+    return head + nb + struct.pack("<%dI" % len(core), *core) + bytes(packed) + b"\xff" * len(seq) + b"".join(fields)
+
+
+def mm_for(seq, rev, lists):
+    """MM text and ML values for calls given in read orientation.
+
+    seq: the stored (reference-orientation) SEQ; rev: the record is reverse (the read is the reverse complement of seq).
+    lists: [(header, calls)] with header such as "C+m?" or "C+hm." and calls [(read position, prob or (prob per code))],
+    every position a base of the list's fundamental base in read orientation (any base for N). The deltas count exact
+    base letters only, as the MM spec does; probabilities of a multi-code list are interleaved per call."""
+    read = revcomp(seq) if rev else seq
+    texts, ml = [], []
+    for header, calls in lists:
+        base = header[0]
+        occ = [i for i, c in enumerate(read) if base == "N" or c.upper() == base]
+        rank = {q: k for k, q in enumerate(occ)}
+        last, deltas = -1, []
+        for q, p in sorted(calls, key=lambda c: c[0]):
+            k = rank[q]
+            deltas.append(k - last - 1)
+            last = k
+            ml += list(p) if isinstance(p, (tuple, list)) else [p]
+        texts.append(header + "".join("," + str(d) for d in deltas) + ";")
+    return "".join(texts), ml
+
+
+def write_fasta(path, contigs, width=60):
+    """FASTA of {name: sequence} plus its samtools-style .fai (name, length, offset, bases and bytes per line)."""
+    with open(path, "w") as fa, open(path + ".fai", "w") as fai:
+        off = 0
+        for name, s in contigs.items():
+            head = ">%s\n" % name
+            off += len(head)
+            fai.write("%s\t%d\t%d\t%d\t%d\n" % (name, len(s), off, width, width + 1))
+            body = "".join(s[i:i + width] + "\n" for i in range(0, len(s), width))
+            fa.write(head + body)
+            off += len(body)
+
+
+def bam_of(refs, records, header_text=b""):
+    """A Bam of [(name, length)] refs and raw records, sorted by (tid, pos) the way a coordinate-sorted BAM is
+    (unplaced records last); write it with .write(path, index=True)."""
+    b = Bam()
+    b.refs = list(refs)
+    b.header_text = header_text or ("@HD\tVN:1.6\tSO:coordinate\n" + "".join("@SQ\tSN:%s\tLN:%d\n" % r for r in refs)).encode()
+    key = lambda r: (struct.unpack_from("<i", r, 0)[0] % (1 << 31), struct.unpack_from("<i", r, 4)[0])
+    b.records = sorted(records, key=key)
+    return b
