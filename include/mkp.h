@@ -108,7 +108,8 @@ typedef struct {
 
 typedef struct {          /* per-chunk counters, filled by mkp_pileup_* */
     uint64_t n_rows;
-    uint64_t n_hot;           /* positions that received a counter slot            */
+    uint64_t n_hot;           /* counter slots: (position, reference strand) pairs;
+                                 pileup-hemi: + strand motif positions              */
     uint64_t n_calls;         /* projected base-mod calls                           */
     uint32_t n_reads_used;    /* reads that produced mod calls (ReadCache "used")   */
     uint32_t n_reads_skipped; /* admitted reads without usable mod info (skip_set)  */

@@ -61,7 +61,7 @@ struct mkp_ctx {
     uint32_t max_ncigar = 1, max_blocks = 1;
     uint64_t heap_bytes = 0;
     // work buffers
-    DevBuf d_rl, d_meta, d_P, d_calls, d_hot, d_hot_prefix, d_block_sums, d_small, d_scr_cq, d_scr_cr, d_slow;
+    DevBuf d_rl, d_meta, d_P, d_calls, d_hot, d_hot_prefix, d_wrec, d_block_sums, d_small, d_scr_cq, d_scr_cr, d_slow;
     DevBuf d_obs_word, d_slots, d_row_counts, d_row_prefix, d_rows, d_hist, d_take;
     // device ingest (BGZF file, inflated BAM stream, record table, slicing scratch)
     DevBuf d_file, d_members, d_bam, d_seeds, d_seg_counts, d_seg_base, d_recs, d_ids, d_plan, d_need, d_totals, d_slab_work;
@@ -172,7 +172,7 @@ void mkp_destroy(mkp_ctx* ctx) {
                                            ctx->slice_prof[0], ctx->slice_prof[1], ctx->slice_prof[2], ctx->slice_prof[3], ctx->slice_prof[4], ctx->slice_prof[5]);
     if (getenv("MKP_TRACE_SLICE")) fprintf(stderr, "[mkp] pass phases (s): buffers %.4f launches %.4f wait %.4f calls %.0f\n", ctx->pass_prof[0], ctx->pass_prof[1], ctx->pass_prof[2], ctx->pass_prof[3]);
     DevBuf* bufs[] = {&ctx->d_hdrs, &ctx->d_heap, &ctx->d_entry_off, &ctx->d_focus_pos, &ctx->d_focus_neg, &ctx->d_rl, &ctx->d_meta, &ctx->d_P,
-                      &ctx->d_calls, &ctx->d_hot, &ctx->d_hot_prefix, &ctx->d_block_sums, &ctx->d_small, &ctx->d_scr_cq, &ctx->d_scr_cr, &ctx->d_slow,
+                      &ctx->d_calls, &ctx->d_hot, &ctx->d_hot_prefix, &ctx->d_wrec, &ctx->d_block_sums, &ctx->d_small, &ctx->d_scr_cq, &ctx->d_scr_cr, &ctx->d_slow,
                       &ctx->d_obs_word, &ctx->d_slots, &ctx->d_row_counts, &ctx->d_row_prefix, &ctx->d_rows, &ctx->d_hist, &ctx->d_take,
                       &ctx->d_file, &ctx->d_members, &ctx->d_bam, &ctx->d_seeds, &ctx->d_seg_counts, &ctx->d_seg_base, &ctx->d_recs, &ctx->d_ids, &ctx->d_plan,
                       &ctx->d_need, &ctx->d_totals, &ctx->d_slab_work, &ctx->d_pscr, &ctx->d_inftab, &ctx->d_tiles, &ctx->d_order,
@@ -259,8 +259,9 @@ static int prepare_decode(mkp_ctx* ctx, ChunkDev* C, int grid) {
     CK(ctx->d_rl.ensure(std::max<size_t>(1, ctx->n_reads) * sizeof(ReadLists)));
     CK(ctx->d_P.ensure(std::max<uint64_t>(1, ctx->total_entries) * 4));
     CK(ctx->d_calls.ensure(std::max<uint64_t>(1, ctx->total_entries) * 8));
-    CK(ctx->d_hot.ensure((size_t)ctx->n_words * 4 + 4));
-    CK(ctx->d_hot_prefix.ensure((size_t)ctx->n_words * 4 + 4));
+    CK(ctx->d_hot.ensure((size_t)ctx->n_words * 8 + 4));
+    CK(ctx->d_hot_prefix.ensure((size_t)ctx->n_words * 8 + 4));
+    CK(ctx->d_wrec.ensure((size_t)ctx->n_words * 16 + 16));
     CK(ctx->d_small.ensure(SMALL_BYTES));
     CK(ctx->d_scr_cq.ensure(nwarps * ((size_t)ctx->max_ncigar + 4) * 4));
     CK(ctx->d_scr_cr.ensure(nwarps * ((size_t)ctx->max_ncigar + 4) * 4));
@@ -311,18 +312,22 @@ static int finish_upload(mkp_ctx* ctx) {
         ctx->order_ready = true;
     }
     if (!ctx->have_focus) { CK(cudaStreamSynchronize(st)); CK(cudaGetLastError()); return 0; }
+    // counter slot of every (focus position, strand): its rank in the [2][n_words] pair (focus_pos, focus_neg)
     const uint32_t n_words = ctx->n_words;
-    const uint32_t n_blk = (n_words + 1023) / 1024;
-    CK(ctx->d_hot.ensure((size_t)n_words * 4 + 4));
-    CK(ctx->d_hot_prefix.ensure((size_t)n_words * 4 + 4));
+    const uint32_t n_blk = (2 * n_words + 1023) / 1024;
+    CK(ctx->d_hot.ensure((size_t)n_words * 8 + 4));
+    CK(ctx->d_hot_prefix.ensure((size_t)n_words * 8 + 4));
+    CK(ctx->d_wrec.ensure((size_t)n_words * 16 + 16));
     CK(ctx->d_block_sums.ensure((size_t)n_blk * 4 + 4));
     CK(ctx->d_small.ensure(SMALL_BYTES));
     uint32_t* u = (uint32_t*)(ctx->d_small.as<uint8_t>() + 34 * 8);
+    CK(cudaMemcpyAsync(ctx->d_hot.p, ctx->d_focus_pos.p, (size_t)n_words * 4, cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(ctx->d_hot.as<uint32_t>() + n_words, ctx->d_focus_neg.p, (size_t)n_words * 4, cudaMemcpyDeviceToDevice, st));
     ctx->launches += 4;
-    k_focus_union<<<(n_words + 255) / 256, 256, 0, st>>>(ctx->d_focus_pos.as<uint32_t>(), ctx->d_focus_neg.as<uint32_t>(), ctx->d_hot.as<uint32_t>(), n_words);
-    k_block_popc<<<n_blk, 1024, 0, st>>>(ctx->d_hot.as<uint32_t>(), n_words, ctx->d_block_sums.as<uint32_t>(), nullptr, nullptr);
+    k_block_popc<<<n_blk, 1024, 0, st>>>(ctx->d_hot.as<uint32_t>(), 2 * n_words, ctx->d_block_sums.as<uint32_t>(), nullptr, nullptr);
     k_scan_blocks<<<1, 1024, 0, st>>>(ctx->d_block_sums.as<uint32_t>(), n_blk, u + 2);
-    k_word_prefix<<<n_blk, 1024, 0, st>>>(ctx->d_hot.as<uint32_t>(), n_words, ctx->d_block_sums.as<uint32_t>(), ctx->d_hot_prefix.as<uint32_t>());
+    k_word_prefix<<<n_blk, 1024, 0, st>>>(ctx->d_hot.as<uint32_t>(), 2 * n_words, ctx->d_block_sums.as<uint32_t>(), ctx->d_hot_prefix.as<uint32_t>());
+    k_word_record<<<(n_words + 255) / 256, 256, 0, st>>>(ctx->d_hot.as<uint32_t>(), ctx->d_hot_prefix.as<uint32_t>(), n_words, ctx->d_wrec.as<uint4>());
     uint32_t n_hot = 0;
     CK(cudaMemcpyAsync(&n_hot, u + 2, 4, cudaMemcpyDeviceToHost, st));
     ctx->n_tiles = ctx->n_reads ? (uint32_t)((ctx->heap_bytes + TL_WIN - 1) / TL_WIN) : 0;
@@ -374,7 +379,7 @@ static int pileup_fused(mkp_ctx* ctx, mkp_stats* stats) {
     bool fused_ran = false;
     for (int attempt = 0;; attempt++) {
         const uint32_t S_cap = ctx->state_cap;
-        const uint32_t stride = SL_MOD + 2 * S_cap;
+        const uint32_t stride = SL_MOD + S_cap;
         CK(ctx->d_slots.ensure(std::max<size_t>(1, n_hot) * stride * 4));
         if (!ctx->d_rows.p) CK(ctx->d_rows.ensure(std::max<size_t>(1024, (size_t)n_hot * 3) * sizeof(mkp_row)));
         ctx->pass_prof[0] += since(tp); tp = now();
@@ -387,7 +392,7 @@ static int pileup_fused(mkp_ctx* ctx, mkp_stats* stats) {
         memset(&F, 0, sizeof F);
         F.hdrs = C.hdrs; F.heap = C.heap; F.n_reads = C.n_reads; F.cs = C.cs; F.ce = C.ce;
         F.read_counter = u + 12;
-        F.focus_pos = C.focus_pos; F.focus_neg = C.focus_neg; F.hot = C.hot; F.hot_prefix = C.hot_prefix;
+        F.rec = ctx->d_wrec.as<uint4>();
         F.slots = ctx->d_slots.as<uint32_t>(); F.stride = stride; F.n_states = S_cap; F.n_words = n_words;
         F.obs_word = ctx->d_obs_word.as<uint32_t>();
         F.states = C.states; F.n_states_seen = C.n_states; F.err = C.err;
@@ -396,7 +401,7 @@ static int pileup_fused(mkp_ctx* ctx, mkp_stats* stats) {
         C.mode = MODE_PILEUP;
         CountDev D;
         D.hdrs = C.hdrs; D.heap = C.heap; D.meta = C.meta; D.calls = C.calls; D.n_reads = C.n_reads; D.cs = C.cs; D.ce = C.ce;
-        D.focus_pos = C.focus_pos; D.focus_neg = C.focus_neg; D.hot = C.hot; D.hot_prefix = C.hot_prefix;
+        D.rec = F.rec;
         D.slots = F.slots; D.stride = stride; D.n_states = S_cap; D.n_words = n_words; D.obs_word = F.obs_word; D.work = u + 6;
         D.order = nullptr;          // (the counting kernels keep the coordinate order: neighbouring reads update neighbouring slots)
         if (use_fused) {
@@ -445,7 +450,7 @@ static int pileup_fused(mkp_ctx* ctx, mkp_stats* stats) {
             CK(cudaEventRecord(ctx->ev[4], st));
         }
         RowDev R;
-        R.hot = C.hot; R.hot_prefix = C.hot_prefix; R.n_words = n_words; R.cs = C.cs; R.ce = C.ce;
+        R.rec = F.rec; R.n_words = n_words; R.cs = C.cs; R.ce = C.ce;
         R.slots = F.slots; R.stride = stride; R.n_states = S_cap; R.states = C.states; R.numeric_mode = ctx->params.numeric_mode;
         R.obs_word = F.obs_word;
         R.row_counts = ctx->d_row_counts.as<uint32_t>(); R.row_prefix = ctx->d_row_prefix.as<uint32_t>();
@@ -522,7 +527,7 @@ int mkp_pileup_resident(mkp_ctx* ctx, mkp_stats* stats) {
     // events: 0 start | 1 after parse | 2 after resolve | 3 after rank | 4 before counts | 5 after count_calls |
     //         6 after count_bases | 7 after row count+scan | 8 before emit | 9 end
     CK(cudaEventRecord(ctx->ev[0], st));
-    CK(cudaMemsetAsync(ctx->d_hot.p, 0, (size_t)n_words * 4, st));
+    CK(cudaMemsetAsync(ctx->d_hot.p, 0, (size_t)n_words * 8, st));
     CK(cudaMemsetAsync(ctx->d_small.p, 0xff, 32 * 8, st));
     CK(cudaMemsetAsync(ctx->d_small.as<uint8_t>() + 32 * 8, 0, SMALL_BYTES - 32 * 8, st));
     C.mode = MODE_PILEUP;
@@ -530,10 +535,14 @@ int mkp_pileup_resident(mkp_ctx* ctx, mkp_stats* stats) {
     CK(cudaEventRecord(ctx->ev[1], st));
     ctx->launches += 2; if (ctx->n_reads) { k_resolve<MODE_PILEUP, true><<<grid, 128, 0, st>>>(C); k_resolve<MODE_PILEUP, false><<<grid, 128, 0, st>>>(C); }
     CK(cudaEventRecord(ctx->ev[2], st));
+    // counter slot of every marked (position, strand): its rank in the [2][n_words] per-strand marks
     uint32_t* u = (uint32_t*)(ctx->d_small.as<uint8_t>() + 34 * 8);   // n_states, err, n_hot, n_rows
-    ctx->launches += 1; k_block_popc<<<n_blk, 1024, 0, st>>>(C.hot, n_words, ctx->d_block_sums.as<uint32_t>(), C.focus_pos, C.focus_neg);
-    ctx->launches += 1; k_scan_blocks<<<1, 1024, 0, st>>>(ctx->d_block_sums.as<uint32_t>(), n_blk, u + 2);
-    ctx->launches += 1; k_word_prefix<<<n_blk, 1024, 0, st>>>(C.hot, n_words, ctx->d_block_sums.as<uint32_t>(), C.hot_prefix);
+    const uint32_t n_blk2 = (2 * n_words + 1023) / 1024;
+    CK(ctx->d_block_sums.ensure((size_t)n_blk2 * 4 + 4));
+    ctx->launches += 1; k_block_popc<<<n_blk2, 1024, 0, st>>>(C.hot, 2 * n_words, ctx->d_block_sums.as<uint32_t>(), C.focus_pos, C.focus_neg);
+    ctx->launches += 1; k_scan_blocks<<<1, 1024, 0, st>>>(ctx->d_block_sums.as<uint32_t>(), n_blk2, u + 2);
+    ctx->launches += 1; k_word_prefix<<<n_blk2, 1024, 0, st>>>(C.hot, 2 * n_words, ctx->d_block_sums.as<uint32_t>(), C.hot_prefix);
+    ctx->launches += 1; k_word_record<<<(n_words + 255) / 256, 256, 0, st>>>(C.hot, C.hot_prefix, n_words, ctx->d_wrec.as<uint4>());
     CK(cudaEventRecord(ctx->ev[3], st));
     uint32_t h_small[4];
     unsigned long long h_calls = 0;
@@ -545,14 +554,14 @@ int mkp_pileup_resident(mkp_ctx* ctx, mkp_stats* stats) {
         if (stats) { memset(stats, 0, sizeof *stats); stats->device_error = derr; }
         return fail(ctx, "device decode error: " + derr_text(derr), -10);
     }
-    const uint32_t stride = SL_MOD + 2 * std::max<uint32_t>(n_states, 1);
+    const uint32_t stride = SL_MOD + std::max<uint32_t>(n_states, 1);
     CK(ctx->d_slots.ensure(std::max<size_t>(1, n_hot) * stride * 4));
     CK(cudaMemsetAsync(ctx->d_slots.p, 0, (size_t)n_hot * stride * 4, st));
     CK(ctx->d_obs_word.ensure((size_t)n_words * 8 + 8));
     CK(cudaMemsetAsync(ctx->d_obs_word.p, 0, (size_t)n_words * 8, st));
     CountDev D;
     D.hdrs = C.hdrs; D.heap = C.heap; D.meta = C.meta; D.calls = C.calls; D.n_reads = C.n_reads; D.cs = C.cs; D.ce = C.ce;
-    D.focus_pos = C.focus_pos; D.focus_neg = C.focus_neg; D.hot = C.hot; D.hot_prefix = C.hot_prefix;
+    D.rec = ctx->d_wrec.as<uint4>();
     D.slots = ctx->d_slots.as<uint32_t>(); D.stride = stride; D.n_states = std::max<uint32_t>(n_states, 1);
     D.n_words = n_words; D.obs_word = ctx->d_obs_word.as<uint32_t>(); D.work = u + 6;
     D.list = nullptr; D.list_count = nullptr; D.order = nullptr;      // (the counting kernels keep the coordinate order: neighbouring reads update neighbouring slots)
@@ -569,7 +578,7 @@ int mkp_pileup_resident(mkp_ctx* ctx, mkp_stats* stats) {
     CK(cudaStreamWaitEvent(st, ctx->ev_join, 0));
     CK(cudaEventRecord(ctx->ev[6], st));
     RowDev R;
-    R.hot = C.hot; R.hot_prefix = C.hot_prefix; R.n_words = n_words; R.cs = C.cs; R.ce = C.ce;
+    R.rec = D.rec; R.n_words = n_words; R.cs = C.cs; R.ce = C.ce;
     R.slots = D.slots; R.stride = stride; R.n_states = D.n_states; R.states = C.states; R.numeric_mode = ctx->params.numeric_mode;
     R.obs_word = D.obs_word;
     R.row_counts = ctx->d_row_counts.as<uint32_t>(); R.row_prefix = ctx->d_row_prefix.as<uint32_t>(); R.rows = nullptr;
@@ -642,7 +651,7 @@ int mkp_hemi_resident(mkp_ctx* ctx, const uint32_t* interval_starts, uint32_t n_
     CK(ctx->d_row_counts.ensure((size_t)n_words * 4 + 4));
     CK(ctx->d_row_prefix.ensure((size_t)n_words * 4 + 4));
     CK(ctx->d_iv_start.ensure((size_t)n_intervals * 4));
-    CK(ctx->d_hemi_hot.ensure((size_t)n_words * 4 + 4));
+    CK(ctx->d_hemi_hot.ensure((size_t)n_words * 8 + 4));        // k_resolve's per-strand marks (not used by the hemi counters)
     CK(ctx->d_hemi_prefix.ensure((size_t)n_words * 4 + 4));
     C.hot = ctx->d_hemi_hot.as<uint32_t>();
     uint32_t* const focus = ctx->d_focus_pos.as<uint32_t>();
@@ -652,7 +661,7 @@ int mkp_hemi_resident(mkp_ctx* ctx, const uint32_t* interval_starts, uint32_t n_
     //         | 8 before emit | 9 end
     CK(cudaEventRecord(ctx->ev[0], st));
     CK(cudaMemcpyAsync(ctx->d_iv_start.p, interval_starts, (size_t)n_intervals * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(C.hot, 0, (size_t)n_words * 4, st));
+    CK(cudaMemsetAsync(C.hot, 0, (size_t)n_words * 8, st));
     CK(cudaMemsetAsync(ctx->d_small.p, 0xff, 32 * 8, st));
     CK(cudaMemsetAsync(ctx->d_small.as<uint8_t>() + 32 * 8, 0, SMALL_BYTES - 32 * 8, st));
     C.mode = MODE_PILEUP;

@@ -55,8 +55,7 @@ struct FusedDev {
     const uint8_t* heap;
     uint32_t n_reads, cs, ce;
     uint32_t* read_counter;                                 // reads are handed to the CTAs in runs of 32
-    const uint32_t* focus_pos; const uint32_t* focus_neg;
-    const uint32_t* hot; const uint32_t* hot_prefix;        // hot = focus_pos | focus_neg, rank structure built at upload
+    const uint4* rec;                                       // per bitmap word: focus bits and slots per strand, built at upload
     uint32_t* slots; uint32_t stride, n_states;             // n_states = state capacity of the slot layout
     uint32_t n_words;
     uint32_t* obs_word;
@@ -98,11 +97,6 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* b, uint32_t parity
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, unsigned long long* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-
-__global__ void k_focus_union(const uint32_t* __restrict__ a, const uint32_t* __restrict__ b, uint32_t* __restrict__ o, uint32_t n) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) o[i] = a[i] | b[i];
 }
 
 __device__ __forceinline__ int state_id_fz(const FusedDev& F, StateCache& sc, int pb, uint32_t code) {
@@ -566,20 +560,21 @@ __device__ __forceinline__ void fused_read(const FusedDev& F, FzWarp& W, StateCa
         if (ra >= rb) return;
         const uint32_t wl = (ra - F.cs + 31) >> 5, wh = (rb - F.cs) >> 5;
         for (uint32_t w = wl + lane; w < wh; w += 32) {
-            if (!F.hot[w]) continue;                        // a word without focus positions produces no rows
+            const uint4 wr = F.rec[w];
+            if (!(wr.x | wr.y)) continue;                   // a word without focus positions produces no rows
             if (pm && (F.obs_word[w] & pm) != pm) atomicOr(&F.obs_word[w], pm);
             if (nm && (F.obs_word[F.n_words + w] & nm) != nm) atomicOr(&F.obs_word[F.n_words + w], nm);
         }
         auto partial = [&](uint32_t pa, uint32_t pb) {
             if (pa >= pb) return;
             const uint32_t w = (pa - F.cs) >> 5, wbase = F.cs + (w << 5);
-            const uint32_t word = F.hot[w];
-            uint32_t bits = word & (FULL << (pa - wbase));
+            const uint4 r = F.rec[w];
+            uint32_t bits = (r.x | r.y) & (FULL << (pa - wbase));
             if (pb < wbase + 32) bits &= (1u << (pb - wbase)) - 1u;
             if ((bits >> lane) & 1u) {
-                uint32_t* S = F.slots + (size_t)(F.hot_prefix[w] + __popc(word & ((1u << lane) - 1u))) * F.stride;
-                if (pm && (S[SL_OBS] & pm) != pm) atomicOr(&S[SL_OBS], pm);
-                if (nm && (S[SL_OBS + 1] & nm) != nm) atomicOr(&S[SL_OBS + 1], nm);
+                const uint32_t kp = pm ? wslot(r, 0, lane) : 0xffffffffu, kn = nm ? wslot(r, 1, lane) : 0xffffffffu;
+                if (kp != 0xffffffffu) { uint32_t* S = F.slots + (size_t)kp * F.stride; if ((S[SL_OBS] & pm) != pm) atomicOr(&S[SL_OBS], pm); }
+                if (kn != 0xffffffffu) { uint32_t* S = F.slots + (size_t)kn * F.stride; if ((S[SL_OBS] & nm) != nm) atomicOr(&S[SL_OBS], nm); }
             }
         };
         if (wl > wh) partial(ra, rb);
@@ -665,8 +660,8 @@ __device__ __forceinline__ void fused_read(const FusedDev& F, FzWarp& W, StateCa
                                 const uint32_t rel = rpos - F.cs;
                                 atomicOr(&W.u.w.mask[(rel >> 5) - wt], 1u << (rel & 31));
                                 n_calls++;
-                                const uint32_t hw = F.hot[rel >> 5];
-                                if ((hw >> (rel & 31)) & 1u) {
+                                const uint4 wr = F.rec[rel >> 5];
+                                if (((wr.x | wr.y) >> (rel & 31)) & 1u) {
                                     // probabilities -> collapse -> call (src/mod_bam.rs:558-600, src/threshold_mod_caller.rs:28-63)
                                     float p0 = __fdiv_rn(__fadd_rn((float)m0[(size_t)j * two], 0.5f), 256.0f), p1 = 0.f;
                                     uint32_t c0 = T.code[lp][0], c1 = 0;
@@ -706,10 +701,8 @@ __device__ __forceinline__ void fused_read(const FusedDev& F, FzWarp& W, StateCa
                                     }
                                     if (cp >= base_thr && (!have || cp >= best)) { have = true; state = 1; }
                                     if (!have) state = 0;
-                                    uint32_t fp = F.focus_pos[rel >> 5], fn = F.focus_neg[rel >> 5];
-                                    uint32_t* S = F.slots + (size_t)(F.hot_prefix[rel >> 5] + __popc(hw & ((1u << (rel & 31)) - 1u))) * F.stride;
                                     if (state < 2 || state - 2 < F.n_states)
-                                        add_feature(S, F.n_states, a, (uint32_t)b, state, (fp >> (rel & 31)) & 1u, (fn >> (rel & 31)) & 1u, 1u);
+                                        add_feature(F.slots, F.stride, wr, rel & 31, a, (uint32_t)b, state, 1u);
                                 }
                             }
                             const uint32_t nt = __popc(tm);
@@ -722,17 +715,14 @@ __device__ __forceinline__ void fused_read(const FusedDev& F, FzWarp& W, StateCa
                     __syncwarp();
                 }
                 if (w > w_last) continue;
-                const uint32_t word = F.hot[w];
-                if (!word) continue;
+                const uint4 wr = F.rec[w];
+                const uint32_t ok = a == 0 ? wr.x : wr.y, pre = a == 0 ? wr.z : wr.w;     // positions with a slot on the read's strand
+                if (!ok) continue;
                 const uint32_t wbase = F.cs + (w << 5);
-                uint32_t bits = word & ~called;
+                uint32_t bits = ok & ~called;
                 if (blo > wbase) bits &= FULL << (blo - wbase);
                 if (bhi < wbase + 32) bits &= (1u << (bhi - wbase)) - 1u;
                 if (!bits) continue;
-                const uint32_t ok = a == 0 ? F.focus_pos[w] : F.focus_neg[w];
-                bits &= ok;
-                if (!bits) continue;
-                const uint32_t pre = F.hot_prefix[w];
                 uint32_t j = 0;
                 {
                     const uint32_t r = wbase + (uint32_t)__ffs(bits) - 1u;
@@ -746,12 +736,12 @@ __device__ __forceinline__ void fused_read(const FusedDev& F, FzWarp& W, StateCa
                     while (W.u.w.r[j + 1] <= r) j++;
                     const uint32_t jc = W.u.w.op[j], jop = jc & 15;
                     if (!(jop == 0 || jop == 7 || jop == 8 || jop == 2)) continue;
-                    uint32_t* S = F.slots + (size_t)(pre + __popc(word & ((1u << bit) - 1u))) * F.stride;
-                    if (jop == 2) { atomicAdd(&S[SL_DEL + a], 1u); continue; }
+                    uint32_t* S = F.slots + (size_t)(pre + __popc(ok & ((1u << bit) - 1u))) * F.stride;
+                    if (jop == 2) { atomicAdd(&S[SL_DEL], 1u); continue; }
                     const uint32_t q = W.u.w.q[j] + (r - W.u.w.r[j]);
                     const int nb = nib_to_base(seq_nibble(seq, q));
                     if (nb > 3) continue;
-                    atomicAdd(&S[SL_BASE + a * 4 + (a ? 3 - nb : nb)], 1u);
+                    atomicAdd(&S[SL_BASE + (a ? 3 - nb : nb)], 1u);
                 }
             }
         }

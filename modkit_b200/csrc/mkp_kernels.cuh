@@ -34,13 +34,13 @@ constexpr int CQ_CAP = MKP_CQ_CAP;  // CIGAR ops whose prefix sums fit in shared
 constexpr int QT_CAP = 512;         // buckets of the query -> op table
 constexpr uint32_t FULL = 0xffffffffu;
 
-// slot layout (u32 words)
-constexpr int SL_BASE = 0;    // [a][b] 8 words, signed
-constexpr int SL_DEL = 8;     // [a]
-constexpr int SL_FILT = 10;   // [s]
-constexpr int SL_CANON = 12;  // [s][pb]
-constexpr int SL_OBS = 20;    // pos mask, neg mask
-constexpr int SL_MOD = 22;    // [s][state]
+// layout (u32 words) of the counter slot of one (position, reference strand) pair; stride SL_MOD + states
+constexpr int SL_BASE = 0;    // [b] 4 words, signed
+constexpr int SL_DEL = 4;
+constexpr int SL_FILT = 5;
+constexpr int SL_CANON = 6;   // [pb]
+constexpr int SL_OBS = 10;    // observed-code mask
+constexpr int SL_MOD = 11;    // [state]
 
 struct DevParams {
     float default_thr;
@@ -78,7 +78,7 @@ struct ChunkDev {
     ReadMeta* meta;
     uint32_t* P;                // forward positions per raw entry
     uint2* calls;               // (ref_pos, info)
-    uint32_t* hot;              // bitmap over [cs,ce)
+    uint32_t* hot;              // [2][n_words] bitmaps over [cs,ce), per reference strand (+ then -)
     uint32_t* hot_prefix;
     unsigned long long* states; // registry: (pb<<32 | code), ~0 empty
     uint32_t* n_states;
@@ -1307,7 +1307,8 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                             calls[n_calls + __popc(em & ((1u << lane) - 1u))] = make_uint2(rpos, info);
                             // marks of a read that fails later stay behind: a hot position without calls yields no rows
                             const uint32_t x = rpos - C.cs;
-                            if (!C.list_mode) atomicOr(&C.hot[x >> 5], 1u << (x & 31));
+                            const uint32_t t = (info & 1u) ^ (rev ? 1u : 0u);        // reference strand of the call
+                            if (!C.list_mode) atomicOr(&C.hot[t * ((C.ce - C.cs + 31) >> 5) + (x >> 5)], 1u << (x & 31));
                         }
                         n_calls += __popc(em);
                     } else {
@@ -1435,7 +1436,10 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                                 if (c_par.edge_on && !(c_par.edge_inv ? (f < c_par.edge_start || f >= L - c_par.edge_end) : (f >= c_par.edge_start && f < L - c_par.edge_end))) continue;
                                 const uint32_t x = r - C.cs;
                                 if (C.focus_pos && !(((C.focus_pos[x >> 5] | C.focus_neg[x >> 5]) >> (x & 31)) & 1u)) continue;
-                                atomicOr(&C.hot[x >> 5], 1u << (x & 31));
+                                // the table of mod strand s counts on reference strand s ^ rev
+                                const uint32_t nw = (C.ce - C.cs + 31) >> 5;
+                                for (uint32_t s = 0; s < 2; s++)
+                                    if ((imp_meta[s] >> (8 * b)) & 0x80u) atomicOr(&C.hot[(s ^ (rev ? 1u : 0u)) * nw + (x >> 5)], 1u << (x & 31));
                             }
                         }
                         if (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) qc2 += len;
@@ -1496,7 +1500,8 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
 }
 
 // ---- rank over the hot bitmap -----------------------------------------------------------------------
-// (marks outside the focus set, which k_resolve does not look at, are cleared here)
+// (with focus bitmaps, `bits` is the [2][n_words / 2] per-strand pair: marks outside the strand's focus set, which k_resolve does
+// not look at, are cleared here)
 __global__ void k_block_popc(uint32_t* __restrict__ bits, uint32_t n_words, uint32_t* __restrict__ block_sums,
                              const uint32_t* __restrict__ focus_pos, const uint32_t* __restrict__ focus_neg) {
     __shared__ uint32_t s[32];
@@ -1504,7 +1509,12 @@ __global__ void k_block_popc(uint32_t* __restrict__ bits, uint32_t n_words, uint
     uint32_t v = 0;
     if (i < n_words) {
         uint32_t word = bits[i];
-        if (focus_pos && word) { const uint32_t keep = word & (focus_pos[i] | focus_neg[i]); if (keep != word) bits[i] = keep; word = keep; }
+        if (focus_pos && word) {
+            const uint32_t half = n_words >> 1;
+            const uint32_t keep = word & (i < half ? focus_pos[i] : focus_neg[i - half]);
+            if (keep != word) bits[i] = keep;
+            word = keep;
+        }
         v = __popc(word);
     }
     uint32_t w = __reduce_add_sync(FULL, v);
@@ -1546,14 +1556,28 @@ __global__ void k_word_prefix(const uint32_t* __restrict__ bits, uint32_t n_word
     if (i < n_words) prefix[i] = block_sums[blockIdx.x] + s_w[threadIdx.x >> 5] + inc - v;
 }
 
+// One 16-byte record per bitmap word, so that a counter update needs one load to find its slot: {+ strand bits, - strand bits,
+// slot of the word's first + bit, slot of its first - bit}, from the ranked [2][n_words] per-strand bitmaps (the - strand slots
+// follow all + strand slots).
+__global__ void k_word_record(const uint32_t* __restrict__ bits, const uint32_t* __restrict__ prefix, uint32_t n_words, uint4* __restrict__ rec) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_words) rec[i] = make_uint4(bits[i], bits[n_words + i], prefix[i], prefix[n_words + i]);
+}
+
+// counter slot of (bit `bit` of the word, reference strand t); ~0u: the pair has none
+__device__ __forceinline__ uint32_t wslot(const uint4& r, uint32_t t, uint32_t bit) {
+    const uint32_t bm = t == 0 ? r.x : r.y;
+    if (!((bm >> bit) & 1u)) return 0xffffffffu;
+    return (t == 0 ? r.z : r.w) + __popc(bm & ((1u << bit) - 1u));
+}
+
 struct CountDev {
     const mkp_read_hdr* hdrs;
     const uint8_t* heap;
     const ReadMeta* meta;
     const uint2* calls;
     uint32_t n_reads, cs, ce;
-    const uint32_t* focus_pos; const uint32_t* focus_neg;
-    const uint32_t* hot; const uint32_t* hot_prefix;
+    const uint4* rec;   // per bitmap word (k_word_record)
     uint32_t* slots;
     uint32_t stride;    // words per slot
     uint32_t n_states;
@@ -1565,17 +1589,15 @@ struct CountDev {
     const uint32_t* order; // else: processing order (longest reads first), or null
 };
 
-__device__ __forceinline__ uint32_t slot_of(const CountDev& D, uint32_t x) {
-    uint32_t w = x >> 5;
-    return D.hot_prefix[w] + __popc(D.hot[w] & ((1u << (x & 31)) - 1u));
-}
-
-// FeatureVector::add_feature + Tally::add_feature (src/pileup/mod.rs:176-193, 238-281) as counter updates
-__device__ __forceinline__ void add_feature(uint32_t* S, uint32_t n_states, uint32_t t, uint32_t pb, uint32_t state, bool ok_pos, bool ok_neg, uint32_t delta) {
-    if (!(t == 0 ? ok_pos : ok_neg)) return;
-    if (state == 0) atomicAdd(&S[SL_FILT + t], delta);
-    else if (state == 1) atomicAdd(&S[SL_CANON + t * 4 + pb], delta);
-    else atomicAdd(&S[SL_MOD + t * n_states + (state - 2)], delta);
+// FeatureVector::add_feature + Tally::add_feature (src/pileup/mod.rs:176-193, 238-281) as counter updates, on reference strand t
+// at bit `bit` of the word with record r
+__device__ __forceinline__ void add_feature(uint32_t* slots, uint32_t stride, const uint4& r, uint32_t bit, uint32_t t, uint32_t pb, uint32_t state, uint32_t delta) {
+    const uint32_t k = wslot(r, t, bit);
+    if (k == 0xffffffffu) return;
+    uint32_t* S = slots + (size_t)k * stride;
+    if (state == 0) atomicAdd(&S[SL_FILT], delta);
+    else if (state == 1) atomicAdd(&S[SL_CANON + pb], delta);
+    else atomicAdd(&S[SL_MOD + (state - 2)], delta);
 }
 
 // warp per read, lanes over its call records
@@ -1598,19 +1620,18 @@ __global__ void __launch_bounds__(256) k_count_calls(CountDev D) {
             uint32_t x = c.x - D.cs;
             uint32_t info = c.y;
             uint32_t st = info & 1u, b = (info >> 1) & 3u, state = (info >> 3) & 0xffu, nosub = (info >> 11) & 1u;
-            uint32_t fp = FULL, fn = FULL;
-            if (D.focus_pos) { fp = D.focus_pos[x >> 5]; fn = D.focus_neg[x >> 5]; }
-            bool ok_pos = (fp >> (x & 31)) & 1u, ok_neg = (fn >> (x & 31)) & 1u;
-            const uint32_t hw = D.hot[x >> 5];
-            if (!((hw >> (x & 31)) & 1u)) continue;            // outside the focus set
-            uint32_t* S = D.slots + (size_t)(D.hot_prefix[x >> 5] + __popc(hw & ((1u << (x & 31)) - 1u))) * D.stride;
+            const uint4 r = D.rec[x >> 5];                     // (a pair outside the focus set has no slot)
+            const uint32_t bit = x & 31, t = st == 0 ? a : 1u - a, pbb = st == 0 ? b : 3u - b;
             // cancel what k_count_bases adds for this (read, position): the inferred entry of this table if the
             // table is implicit, else the NoCall base on tally[a] (unless the other strand's table is implicit
             // there, in which case no NoCall is counted, or the '+' record of a +/- pair already cancels it)
             const uint32_t imp_own = (m.imp[st] >> (8 * b)) & 0xffu, imp_other = (m.imp[1 - st] >> (8 * b)) & 0xffu;
-            if (imp_own & 0x80u) add_feature(S, D.n_states, st == 0 ? a : 1u - a, st == 0 ? b : 3u - b, imp_own & 0x7fu, ok_pos, ok_neg, 0xffffffffu);
-            else if (!(m.flags & 4) && !(imp_other & 0x80u) && !nosub && (a == 0 ? ok_pos : ok_neg)) atomicAdd(&S[SL_BASE + a * 4 + b], 0xffffffffu);
-            add_feature(S, D.n_states, st == 0 ? a : 1u - a, st == 0 ? b : 3u - b, state, ok_pos, ok_neg, 1u);
+            if (imp_own & 0x80u) add_feature(D.slots, D.stride, r, bit, t, pbb, imp_own & 0x7fu, 0xffffffffu);
+            else if (!(m.flags & 4) && !(imp_other & 0x80u) && !nosub) {
+                const uint32_t k = wslot(r, a, bit);
+                if (k != 0xffffffffu) atomicAdd(&D.slots[(size_t)k * D.stride + SL_BASE + b], 0xffffffffu);
+            }
+            add_feature(D.slots, D.stride, r, bit, t, pbb, state, 1u);
         }
     }
 }
@@ -1657,13 +1678,13 @@ __global__ void __launch_bounds__(256, MKP_MINB_BASES) k_count_bases(CountDev D)
             auto partial = [&](uint32_t pa, uint32_t pb) {     // [pa,pb) lies inside one bitmap word
                 if (pa >= pb) return;
                 const uint32_t w = (pa - D.cs) >> 5, wbase = D.cs + (w << 5);
-                const uint32_t word = D.hot[w];
-                uint32_t bits = word & (FULL << (pa - wbase));
+                const uint4 r = D.rec[w];
+                uint32_t bits = (r.x | r.y) & (FULL << (pa - wbase));
                 if (pb < wbase + 32) bits &= (1u << (pb - wbase)) - 1u;
                 if ((bits >> lane) & 1u) {
-                    uint32_t* S = D.slots + (size_t)(D.hot_prefix[w] + __popc(word & ((1u << lane) - 1u))) * D.stride;
-                    if (pm && (S[SL_OBS] & pm) != pm) atomicOr(&S[SL_OBS], pm);
-                    if (nm && (S[SL_OBS + 1] & nm) != nm) atomicOr(&S[SL_OBS + 1], nm);
+                    const uint32_t kp = pm ? wslot(r, 0, lane) : 0xffffffffu, kn = nm ? wslot(r, 1, lane) : 0xffffffffu;
+                    if (kp != 0xffffffffu) { uint32_t* S = D.slots + (size_t)kp * D.stride; if ((S[SL_OBS] & pm) != pm) atomicOr(&S[SL_OBS], pm); }
+                    if (kn != 0xffffffffu) { uint32_t* S = D.slots + (size_t)kn * D.stride; if ((S[SL_OBS] & nm) != nm) atomicOr(&S[SL_OBS], nm); }
                 }
             };
             if (wl > wh) partial(ra, rb);                       // the run starts and ends inside one word
@@ -1721,14 +1742,8 @@ __global__ void __launch_bounds__(256, MKP_MINB_BASES) k_count_bases(CountDev D)
                                 if ((rel >> 5) >= wt) atomicOr(&s_mask[wib][(rel >> 5) - wt], 1u << (rel & 31));
 #ifndef MKP_NO_FUSED_CALLS
                                 // the record's own counter (k_count_calls leaves these reads alone): modcall / canonical / filtered
-                                const uint32_t hw = D.hot[rel >> 5];
-                                if ((hw >> (rel & 31)) & 1u) {                       // else: outside the focus set
-                                    uint32_t fp = FULL, fn = FULL;
-                                    if (D.focus_pos) { fp = D.focus_pos[rel >> 5]; fn = D.focus_neg[rel >> 5]; }
-                                    const uint32_t st = info & 1u, cb = (info >> 1) & 3u, state = (info >> 3) & 0xffu;
-                                    uint32_t* S = D.slots + (size_t)(D.hot_prefix[rel >> 5] + __popc(hw & ((1u << (rel & 31)) - 1u))) * D.stride;
-                                    add_feature(S, D.n_states, st == 0 ? a : 1u - a, st == 0 ? cb : 3u - cb, state, (fp >> (rel & 31)) & 1u, (fn >> (rel & 31)) & 1u, 1u);
-                                }
+                                const uint32_t st = info & 1u, cb = (info >> 1) & 3u, state = (info >> 3) & 0xffu;
+                                add_feature(D.slots, D.stride, D.rec[rel >> 5], rel & 31, st == 0 ? a : 1u - a, st == 0 ? cb : 3u - cb, state, 1u);
 #endif
                             }
                             const uint32_t nt = __popc(__ballot_sync(FULL, take));
@@ -1739,20 +1754,18 @@ __global__ void __launch_bounds__(256, MKP_MINB_BASES) k_count_bases(CountDev D)
                         called = s_mask[wib][lane];
                     }
                     if (w > w_last) continue;
-                    const uint32_t word = D.hot[w];
+                    const uint4 wr = D.rec[w];
+                    const uint32_t word = wr.x | wr.y;
                     if (!word) continue;
                     const uint32_t wbase = D.cs + (w << 5);
                     uint32_t bits = word & ~called;
                     if (blo > wbase) bits &= FULL << (blo - wbase);
                     if (bhi < wbase + 32) bits &= (1u << (bhi - wbase)) - 1u;
                     if (!bits) continue;
-                    // positions whose strand rule admits what this read can add there
-                    uint32_t fp = FULL, fn = FULL;
-                    if (D.focus_pos) { fp = D.focus_pos[w]; fn = D.focus_neg[w]; }
-                    const uint32_t ok = a == 0 ? fp : fn;
-                    bits &= has_imp ? (fp | fn) : ok;
+                    // positions with a slot on the read's strand (only implicit tables add to the other strand)
+                    const uint32_t ok = a == 0 ? wr.x : wr.y, pre = a == 0 ? wr.z : wr.w;
+                    if (!has_imp) bits &= ok;
                     if (!bits) continue;
-                    const uint32_t pre = D.hot_prefix[w];
                     // op under the first candidate position: largest j with s_r[j] <= r (ops without reference length share
                     // their start with the next op, so the largest index is the op that holds r)
                     uint32_t j = 0;
@@ -1769,23 +1782,22 @@ __global__ void __launch_bounds__(256, MKP_MINB_BASES) k_count_bases(CountDev D)
                         const uint32_t jc = s_op[wib][j], jop = jc & 15;
                         if (!(jop == 0 || jop == 7 || jop == 8 || jop == 2)) continue;       // reference skip
                         if (jop == 2 && !((ok >> bit) & 1u)) continue;
-                        uint32_t* S = D.slots + (size_t)(pre + __popc(word & ((1u << bit) - 1u))) * D.stride;
-                        if (jop == 2) { atomicAdd(&S[SL_DEL + a], 1u); continue; }
+                        uint32_t* S = D.slots + (size_t)(pre + __popc(ok & ((1u << bit) - 1u))) * D.stride;   // (when ok has the bit)
+                        if (jop == 2) { atomicAdd(&S[SL_DEL], 1u); continue; }
                         const uint32_t q = s_q[wib][j] + (r - s_r[wib][j]);
                         const int nb = nib_to_base(seq_nibble(seq, q));
                         if (nb > 3) continue;
                         const uint32_t b = a ? 3 - nb : nb;
-                        if (!has_imp) { atomicAdd(&S[SL_BASE + a * 4 + b], 1u); continue; }
+                        if (!has_imp) { atomicAdd(&S[SL_BASE + b], 1u); continue; }
                         uint32_t ip = (m.imp[0] >> (8 * b)) & 0xffu, in = (m.imp[1] >> (8 * b)) & 0xffu;
                         if ((ip | in) & 0x80u) {
                             // inferred-canonical entries of implicit tables, subject to the edge filter
                             const uint32_t f = a ? h.l_seq - 1u - q : q;
                             if (c_par.edge_on && !(c_par.edge_inv ? (f < c_par.edge_start || f >= h.l_seq - c_par.edge_end) : (f >= c_par.edge_start && f < h.l_seq - c_par.edge_end))) ip = in = 0;
                         }
-                        const bool okp = (fp >> bit) & 1u, okn = (fn >> bit) & 1u;
-                        if (!((ip | in) & 0x80u)) { if ((ok >> bit) & 1u) atomicAdd(&S[SL_BASE + a * 4 + b], 1u); continue; }
-                        if (ip & 0x80u) add_feature(S, D.n_states, a, b, ip & 0x7fu, okp, okn, 1u);
-                        if (in & 0x80u) add_feature(S, D.n_states, 1u - a, 3u - b, in & 0x7fu, okp, okn, 1u);
+                        if (!((ip | in) & 0x80u)) { if ((ok >> bit) & 1u) atomicAdd(&S[SL_BASE + b], 1u); continue; }
+                        if (ip & 0x80u) add_feature(D.slots, D.stride, wr, bit, a, b, ip & 0x7fu, 1u);
+                        if (in & 0x80u) add_feature(D.slots, D.stride, wr, bit, 1u - a, 3u - b, in & 0x7fu, 1u);
                     }
                 }
             }
@@ -1796,7 +1808,7 @@ __global__ void __launch_bounds__(256, MKP_MINB_BASES) k_count_bases(CountDev D)
 }
 
 struct RowDev {
-    const uint32_t* hot; const uint32_t* hot_prefix;
+    const uint4* rec;         // per bitmap word (k_word_record)
     uint32_t n_words, cs, ce;
     const uint32_t* slots;
     uint32_t stride, n_states;
@@ -1809,64 +1821,63 @@ struct RowDev {
     uint32_t rows_cap;        // emit pass: a word whose rows do not fit is skipped (the host grows the buffer and emits again)
 };
 
-// rows of one slot, in output order. emit == nullptr => count only
-__device__ __forceinline__ uint32_t slot_rows(const RowDev& R, const uint32_t* S, uint32_t pos, uint32_t w, mkp_row* out) {
+// rows of the slot S of (pos, strand s), in output order. emit == nullptr => count only
+__device__ __forceinline__ uint32_t slot_rows(const RowDev& R, const uint32_t* S, uint32_t pos, uint32_t w, uint32_t s, mkp_row* out) {
     uint32_t n = 0;
-    for (uint32_t s = 0; s < 2; s++) {
-        uint32_t mod_by_base[4] = {0, 0, 0, 0};
-        for (uint32_t id = 0; id < R.n_states; id++) mod_by_base[(uint32_t)(R.states[id] >> 32) & 3u] += S[SL_MOD + s * R.n_states + id];
-        const uint32_t obs = S[SL_OBS + s] | R.obs_word[s * R.n_words + w];
-        const uint32_t row0 = n;
-        for (uint32_t pb = 0; pb < 4; pb++) {
-            uint32_t n_can = S[SL_CANON + s * 4 + pb], total_mod = mod_by_base[pb];
-            if (n_can + total_mod == 0) continue;
-            uint32_t n_diff = 0;
-            for (uint32_t b = 0; b < 4; b++) if (b != pb) n_diff += S[SL_BASE + s * 4 + b] + S[SL_CANON + s * 4 + b] + mod_by_base[b];
-            mkp_row r;
-            r.pos = pos; r.strand = s == 0 ? '+' : '-'; r.primary_base = (uint8_t)pb; r.reserved = 0;
-            r.n_canon = n_can; r.n_delete = S[SL_DEL + s]; r.n_filtered = S[SL_FILT + s]; r.n_diff = n_diff; r.n_nocall = S[SL_BASE + s * 4 + pb];
-            if (R.numeric_mode == 1) {
-                r.code = (uint32_t)("ACGT"[pb]); r.n_mod = total_mod; r.n_other = 0;
+    uint32_t mod_by_base[4] = {0, 0, 0, 0};
+    for (uint32_t id = 0; id < R.n_states; id++) mod_by_base[(uint32_t)(R.states[id] >> 32) & 3u] += S[SL_MOD + id];
+    const uint32_t obs = S[SL_OBS] | R.obs_word[s * R.n_words + w];
+    for (uint32_t pb = 0; pb < 4; pb++) {
+        uint32_t n_can = S[SL_CANON + pb], total_mod = mod_by_base[pb];
+        if (n_can + total_mod == 0) continue;
+        uint32_t n_diff = 0;
+        for (uint32_t b = 0; b < 4; b++) if (b != pb) n_diff += S[SL_BASE + b] + S[SL_CANON + b] + mod_by_base[b];
+        mkp_row r;
+        r.pos = pos; r.strand = s == 0 ? '+' : '-'; r.primary_base = (uint8_t)pb; r.reserved = 0;
+        r.n_canon = n_can; r.n_delete = S[SL_DEL]; r.n_filtered = S[SL_FILT]; r.n_diff = n_diff; r.n_nocall = S[SL_BASE + pb];
+        if (R.numeric_mode == 1) {
+            r.code = (uint32_t)("ACGT"[pb]); r.n_mod = total_mod; r.n_other = 0;
+            if (out) out[n] = r;
+            n++;
+        } else {
+            for (uint32_t id = 0; id < R.n_states; id++) {
+                unsigned long long key = R.states[id];
+                if (((uint32_t)(key >> 32) & 3u) != pb || !((obs >> id) & 1u)) continue;
+                uint32_t n_mod = S[SL_MOD + id];
+                r.code = (uint32_t)key; r.n_mod = n_mod; r.n_other = total_mod - n_mod;
                 if (out) out[n] = r;
                 n++;
-            } else {
-                for (uint32_t id = 0; id < R.n_states; id++) {
-                    unsigned long long key = R.states[id];
-                    if (((uint32_t)(key >> 32) & 3u) != pb || !((obs >> id) & 1u)) continue;
-                    uint32_t n_mod = S[SL_MOD + s * R.n_states + id];
-                    r.code = (uint32_t)key; r.n_mod = n_mod; r.n_other = total_mod - n_mod;
-                    if (out) out[n] = r;
-                    n++;
-                }
             }
         }
-        // stable insertion sort of this strand's rows by code (derived Ord: Code(char) < ChEbi == u32 order)
-        if (out) for (uint32_t i = row0 + 1; i < n; i++) {
-            mkp_row key = out[i];
-            uint32_t j = i;
-            while (j > row0 && out[j - 1].code > key.code) { out[j] = out[j - 1]; j--; }
-            out[j] = key;
-        }
+    }
+    // stable insertion sort of this strand's rows by code (derived Ord: Code(char) < ChEbi == u32 order)
+    if (out) for (uint32_t i = 1; i < n; i++) {
+        mkp_row key = out[i];
+        uint32_t j = i;
+        while (j > 0 && out[j - 1].code > key.code) { out[j] = out[j - 1]; j--; }
+        out[j] = key;
     }
     return n;
 }
 
-// thread per hot-bitmap word
+// thread per hot-bitmap word; rows by position, + strand before - strand
 template <bool EMIT>
 __global__ void __launch_bounds__(256) k_rows(RowDev R) {
     uint32_t w = blockIdx.x * blockDim.x + threadIdx.x;
     if (w >= R.n_words) return;
-    uint32_t bits = R.hot[w];
+    const uint4 wr = R.rec[w];
+    uint32_t bits = wr.x | wr.y;
     if (!bits) { if (!EMIT) R.row_counts[w] = 0; return; }
-    uint32_t slot = R.hot_prefix[w];
+    uint32_t slot_p = wr.z, slot_n = wr.w;
     uint32_t n = 0;
     if (EMIT && (unsigned long long)R.row_prefix[w] + R.row_counts[w] > (unsigned long long)R.rows_cap) return;
     mkp_row* out = EMIT ? R.rows + R.row_prefix[w] : nullptr;
     while (bits) {
         uint32_t bit = __ffs(bits) - 1;
         bits &= bits - 1;
-        n += slot_rows(R, R.slots + (size_t)slot * R.stride, R.cs + (w << 5) + bit, w, EMIT ? out + n : nullptr);
-        slot++;
+        const uint32_t pos = R.cs + (w << 5) + bit;
+        if ((wr.x >> bit) & 1u) n += slot_rows(R, R.slots + (size_t)slot_p++ * R.stride, pos, w, 0, EMIT ? out + n : nullptr);
+        if ((wr.y >> bit) & 1u) n += slot_rows(R, R.slots + (size_t)slot_n++ * R.stride, pos, w, 1, EMIT ? out + n : nullptr);
     }
     if (!EMIT) R.row_counts[w] = n;
 }

@@ -418,8 +418,8 @@ __global__ void __launch_bounds__(TL_THREADS, 1) k_pileup_tile(const TileDev Tl)
                     const uint32_t rel = rpos - F.cs;
                     atomicOr(&S.arena[R.called_off + ((rel >> 5) - R.w0)], 1u << (rel & 31));
                     my_calls++;
-                    const uint32_t hw = F.hot[rel >> 5];
-                    if (!((hw >> (rel & 31)) & 1u)) continue;
+                    const uint4 wr = F.rec[rel >> 5];
+                    if (!(((wr.x | wr.y) >> (rel & 31)) & 1u)) continue;
                     float p0 = __fdiv_rn(__fadd_rn((float)m0[(size_t)j * G.two], 0.5f), 256.0f), p1 = 0.f;
                     uint32_t c0 = G.c0, c1 = 0;
                     int n2c = 1;
@@ -458,10 +458,8 @@ __global__ void __launch_bounds__(TL_THREADS, 1) k_pileup_tile(const TileDev Tl)
                     }
                     if (cp >= base_thr && (!have || cp >= best)) { have = true; state = 1; }
                     if (!have) state = 0;
-                    const uint32_t fp = F.focus_pos[rel >> 5], fn = F.focus_neg[rel >> 5];
-                    uint32_t* Sl = F.slots + (size_t)(F.hot_prefix[rel >> 5] + __popc(hw & ((1u << (rel & 31)) - 1u))) * F.stride;
                     if (state < 2 || state - 2 < F.n_states)
-                        add_feature(Sl, F.n_states, a, G.base, state, (fp >> (rel & 31)) & 1u, (fn >> (rel & 31)) & 1u, 1u);
+                        add_feature(F.slots, F.stride, wr, rel & 31, a, G.base, state, 1u);
                 }
             }
             if (my_calls) atomicAdd(&R.n_calls, my_calls);
@@ -481,13 +479,13 @@ __global__ void __launch_bounds__(TL_THREADS, 1) k_pileup_tile(const TileDev Tl)
             const uint32_t pm = R.pm, nm = R.nm;
             for (uint32_t wi = tid; wi < R.nw; wi += TL_THREADS) {
                 const uint32_t w = R.w0 + wi;
-                const uint32_t word = F.hot[w];
+                const uint4 wr = F.rec[w];
+                const uint32_t word = wr.x | wr.y;
                 if (!word) continue;
                 const uint32_t wbase = F.cs + (w << 5);
                 uint32_t in = FULL;                                   // positions of the word inside [ra, rb)
                 if (ra > wbase) in &= FULL << (ra - wbase);
                 if (rb < wbase + 32) in &= (1u << (rb - wbase)) - 1u;
-                const uint32_t pre = F.hot_prefix[w];
                 if (pm | nm) {
                     if (in == FULL) {
                         if (pm && (F.obs_word[w] & pm) != pm) atomicOr(&F.obs_word[w], pm);
@@ -497,13 +495,14 @@ __global__ void __launch_bounds__(TL_THREADS, 1) k_pileup_tile(const TileDev Tl)
                         while (ob) {
                             const uint32_t bit = __ffs(ob) - 1;
                             ob &= ob - 1;
-                            uint32_t* Sl = F.slots + (size_t)(pre + __popc(word & ((1u << bit) - 1u))) * F.stride;
-                            if (pm && (Sl[SL_OBS] & pm) != pm) atomicOr(&Sl[SL_OBS], pm);
-                            if (nm && (Sl[SL_OBS + 1] & nm) != nm) atomicOr(&Sl[SL_OBS + 1], nm);
+                            const uint32_t kp = pm ? wslot(wr, 0, bit) : 0xffffffffu, kn = nm ? wslot(wr, 1, bit) : 0xffffffffu;
+                            if (kp != 0xffffffffu) { uint32_t* Sl = F.slots + (size_t)kp * F.stride; if ((Sl[SL_OBS] & pm) != pm) atomicOr(&Sl[SL_OBS], pm); }
+                            if (kn != 0xffffffffu) { uint32_t* Sl = F.slots + (size_t)kn * F.stride; if ((Sl[SL_OBS] & nm) != nm) atomicOr(&Sl[SL_OBS], nm); }
                         }
                     }
                 }
-                uint32_t bits = word & in & ~S.arena[R.called_off + wi] & (a == 0 ? F.focus_pos[w] : F.focus_neg[w]);
+                const uint32_t ok = a == 0 ? wr.x : wr.y, pre = a == 0 ? wr.z : wr.w;    // positions with a slot on the read's strand
+                uint32_t bits = ok & in & ~S.arena[R.called_off + wi];
                 while (bits) {
                     const uint32_t bit = __ffs(bits) - 1;
                     bits &= bits - 1;
@@ -511,13 +510,13 @@ __global__ void __launch_bounds__(TL_THREADS, 1) k_pileup_tile(const TileDev Tl)
                     uint32_t lo = 0, hi = nc;                         // op holding rp: largest i with reference start <= rp
                     while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (cr[mid] <= rp) lo = mid; else hi = mid; }
                     if (cr[lo + 1] <= rp) continue;                   // (cannot happen inside [ref_start, ref_end))
-                    uint32_t* Sl = F.slots + (size_t)(pre + __popc(word & ((1u << bit) - 1u))) * F.stride;
+                    uint32_t* Sl = F.slots + (size_t)(pre + __popc(ok & ((1u << bit) - 1u))) * F.stride;
                     const uint32_t e = cq[lo];
-                    if (!(e & 1u)) { atomicAdd(&Sl[SL_DEL + a], 1u); continue; }          // a deletion (reference skips were excluded)
+                    if (!(e & 1u)) { atomicAdd(&Sl[SL_DEL], 1u); continue; }          // a deletion (reference skips were excluded)
                     const uint32_t q = (e >> 1) + (rp - cr[lo]);
                     const int nb = nib_to_base(seq_nibble(seq, q));
                     if (nb > 3) continue;
-                    atomicAdd(&Sl[SL_BASE + a * 4 + (a ? 3 - nb : nb)], 1u);
+                    atomicAdd(&Sl[SL_BASE + (a ? 3 - nb : nb)], 1u);
                 }
             }
         }
