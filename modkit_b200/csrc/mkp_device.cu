@@ -1157,4 +1157,16 @@ size_t mkp_algorithmic_bytes(const mkp_chunk* ch, size_t n_rows) {
     return b + 40 * n_rows;
 }
 
+#ifdef MKP_PARSE_CLOCKS
+// Measurement builds only: the k_parse phase counters (mkp_kernels.cuh, g_parse_clk) of the current device, summed since the
+// last reset, into out[0 .. n); reset != 0 zeroes them afterwards. Returns the number of counters.
+int mkp_debug_parse_clocks(unsigned long long* out, int n, int reset) {
+    unsigned long long v[PCLK_N];
+    if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(v, g_parse_clk, sizeof v) != cudaSuccess) return -1;
+    for (int k = 0; k < n && k < PCLK_N; k++) out[k] = v[k];
+    if (reset) { memset(v, 0, sizeof v); if (cudaMemcpyToSymbol(g_parse_clk, v, sizeof v) != cudaSuccess) return -1; }
+    return PCLK_N;
+}
+#endif
+
 }  // extern "C"

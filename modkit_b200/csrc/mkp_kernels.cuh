@@ -373,8 +373,10 @@ __device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t* P, uint32_t 
 
 // Kernel A: per read, everything that depends only on the read's own bytes: admission, reference span, MM list
 // discovery, per-base occurrence counts, MM token parse + select -> forward positions P[] and the list table.
+// k_parse: 9 blocks of 128 threads = 56 registers and no spills. At 10 blocks (48 registers) it spills 72 / 100 bytes and takes
+// 1.4 % longer on an H100; at 8 (63 registers, 32 warps per SM) it took 2 % longer (profiles/README.md)
 #ifndef MKP_MINB_PARSE
-#define MKP_MINB_PARSE 10
+#define MKP_MINB_PARSE 9
 #endif
 #ifndef MKP_MINB_RESOLVE_FAST
 #define MKP_MINB_RESOLVE_FAST 8
@@ -388,15 +390,38 @@ __device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t* P, uint32_t 
 #ifndef MKP_MINB_BASES
 #define MKP_MINB_BASES 5
 #endif
+// MKP_PARSE_CLOCKS=1 (measurement builds only): every warp of k_parse sums clock64() deltas per phase over the reads it handles
+// and adds them into g_parse_clk at exit: [0] queue + header, [1] CIGAR span, [2] MM list scan, [3] alias compare, [4] delta
+// tokenizer, [5] streaming select, [6] hand-over, [7] reads, [8] SEQ rounds of the select. Read back by mkp_debug_parse_clocks.
+#ifdef MKP_PARSE_CLOCKS
+constexpr int PCLK_N = 9;
+__device__ unsigned long long g_parse_clk[PCLK_N];
+// (the sums live in shared memory, so the measured kernel keeps the register budget of the default build)
+#define PCLK_INIT __shared__ unsigned long long s_pclk[4][PCLK_N]; unsigned long long* pclk = s_pclk[wib]; \
+    if (lane < PCLK_N) pclk[lane] = 0; __syncwarp(); unsigned long long pclk_t = clock64()
+#define PCLK(k) do { const unsigned long long t_ = clock64(); if (lane == 0) pclk[k] += t_ - pclk_t; pclk_t = t_; } while (0)
+#define PCLK_COUNT(k, n) do { if (lane == 0) pclk[k] += (n); } while (0)
+#define PCLK_FLUSH do { __syncwarp(); if (lane < PCLK_N) atomicAdd(&g_parse_clk[lane], pclk[lane]); } while (0)
+#else
+#define PCLK_INIT do {} while (0)
+#define PCLK(k) do {} while (0)
+#define PCLK_COUNT(k, n) do {} while (0)
+#define PCLK_FLUSH do {} while (0)
+#endif
+// SEQ per lane and round of k_parse's streaming select, in uint4 (32 bases each). On an H100, 2 took 1.95 ms per pass on the
+// profile chunk and 4 took 2.07 (profiles/README.md): wider blocks cost more in the token lookup than they save in rounds.
+constexpr int SEL_Q = 2;
 __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
     __shared__ ListTab s_tab[4];
     __shared__ __align__(16) uint8_t s_txt[4][160];
     __shared__ uint8_t s_tok[4][132];
-    __shared__ uint32_t s_cb[4][32], s_bm[4][32], s_tp[4][MAX_LISTS];
+    __shared__ uint32_t s_cb[4][32], s_tp[4][MAX_LISTS];
+    __shared__ uint4 s_fq[SEL_Q][4][32];
     __shared__ uint32_t s_val[4][96];
     const uint32_t lane = lane_id();
     const uint32_t wib = threadIdx.x >> 5;
     ListTab& T = s_tab[wib];
+    PCLK_INIT;
 
     for (;;) {
         // dynamic work distribution: reads differ in length by 2-3 orders of magnitude
@@ -407,7 +432,8 @@ __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
             else if (C.order && ri < C.n_reads) ri = C.order[ri];
         }
         ri = __shfl_sync(FULL, ri, 0);
-        if (ri >= C.n_reads) break;
+        if (ri >= C.n_reads) { PCLK(0); break; }
+        PCLK_COUNT(7, 1);
         const mkp_read_hdr h = C.hdrs[ri];
         const uint32_t flag = h.flags & 0xffffu;
         const uint32_t L = h.l_seq;
@@ -420,7 +446,8 @@ __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
         if (C.mode == MODE_PILEUP) admitted = !(flag & (0x4 | 0x100 | 0x200 | 0x400 | 0x800)) && L > 0;
         else admitted = !(flag & (0x100 | 0x400 | 0x800)) && L > 0 && (C.take == nullptr || C.take[ri]) &&
                         !((flag & 0x4) && (!C.hist_include_unaligned || c_par.edge_on));
-        if (!admitted) { if (lane == 0) { C.meta[ri] = meta; C.rl[ri].n = 0; C.rl[ri].flags = 1; } continue; }
+        if (!admitted) { if (lane == 0) { C.meta[ri] = meta; C.rl[ri].n = 0; C.rl[ri].flags = 1; } PCLK(0); continue; }
+        PCLK(0);
         meta.flags = 1;
         const uint32_t* cig = (const uint32_t*)(C.heap + h.off);
         const uint8_t* seq = C.heap + h.off + 4ull * h.n_cigar;
@@ -436,6 +463,7 @@ __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
             }
             meta.ref_end = (int32_t)((uint32_t)h.ref_start + __reduce_add_sync(FULL, rsum));
         }
+        PCLK(1);
         bool err = (h.flags & MKP_RF_TAGS_INVALID) != 0;
         // ---- phase 1: list discovery: warp-parallel scan for ';' and the first ',' of each part; the few
         //      header bytes of each part are parsed by lane 0 (src/mod_bam.rs:900-1000) ------------------
@@ -533,13 +561,13 @@ __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
             int x = rev ? 3 - b : b;
             need |= 1u << x;
         }
-        const uint32_t nblk = (L + 31) >> 5;
         if (lane < 4) T.tot[lane] = 0;
         __syncwarp();
         // ---- phase 3: tokens -> forward positions ------------------------------------------------------
         uint32_t* P = C.P + meta.entry_off;
         uint32_t ent = 0, mlp = 0;
         uint32_t alias_mask = 0;              // lists that share the entries of the list before them
+        PCLK(2);
         for (uint32_t l = 0; l < nl && !err; l++) {
             const uint32_t ds = T.d_start[l], de = T.d_end[l];
             const bool must = T.n_delta[l] == 0xffffffffu;
@@ -566,9 +594,11 @@ __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
                     mlp += ntok * T.ncodes[l];
                     alias_mask |= 1u << l;
                     __syncwarp();
+                    PCLK(3);
                     continue;
                 }
             }
+            PCLK(3);
             // delta values of up to 32 tokens (one per lane, `mine` lanes in token order) -> forward positions P[]
             // delta values of up to 32 tokens (one per lane, `mine` lanes in token order) -> 0-based occurrence index of the
             // list's base in forward-read order (for 'N' lists that already is the forward position); stored in P[] and
@@ -724,14 +754,21 @@ __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
             mlp += ntok * T.ncodes[l];
             ent += ntok;
             __syncwarp();
+            PCLK(4);
         }
-        // ---- streaming select: for every needed base, one pass over the SEQ in forward-read order (32 bases per lane:
-        //      occurrence mask by SWAR nibble compare, warp scan of the popcounts) during which the tokens of all lists of
-        //      that base are placed: a token with occurrence index k lands in the block whose running count brackets k
-        //      (5-step search over the 32 counts in shared memory), at the (k - count)-th set bit of its mask.
+        // ---- streaming select: for every needed base, one pass over the SEQ in forward-read order during which the tokens of
+        //      all lists of that base are placed. The SEQ is read in blocks of SEL_Q uint4 (32 SEL_Q bases) of the 16-byte
+        //      aligned grid that holds it (block b starts at query base 32 SEL_Q b - 2 a, a = seq & 15), one block per lane and
+        //      32 per round; only the first and the last round mask the bytes outside the SEQ. Per lane: the nibble-equality
+        //      flags (bit 4n) of its words and a warp scan of their popcounts. A token with occurrence index k lands in the
+        //      block whose running count brackets k (5-step search over the 32 counts in shared memory), at the (k - count)-th
+        //      match of the block, looked up in the one word that holds it. The pass is bound by instruction issue, not by its
+        //      loads, so the blocks are as wide as the registers allow: every round pays one scan and one token placement.
         if (!err && need) {
-            const uint32_t* seqw = (const uint32_t*)seq;   // 4-byte aligned
-            const uint32_t nbytes = (L + 1) >> 1;
+            const uint32_t a16 = (uint32_t)((uintptr_t)seq & 15u);
+            const uint4* seq4 = (const uint4*)(seq - a16);
+            const uint32_t s_end = a16 + ((L + 1) >> 1);                 // the SEQ is bytes [a16, s_end) of the grid
+            const uint32_t nb = (s_end + 16 * SEL_Q - 1) / (16 * SEL_Q);
             for (int x = 0; x < 4 && !err; x++) {
                 if (!(need & (1u << x))) continue;
                 const int bfw = rev ? 3 - x : x;                        // forward base of this nibble
@@ -744,30 +781,83 @@ __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
                 lists &= ~alias_mask;                                    // shared entries are placed once, by their first list
                 if (lane < MAX_LISTS) s_tp[wib][lane] = 0;
                 __syncwarp();
+                // The first list of the base keeps its window of 32 occurrence indices in registers (wv, one per lane) across
+                // rounds; P is read again only when a window has been placed. Other lists of the base (their deltas differ from
+                // it) read theirs from P every round.
+                const uint32_t n0 = lists ? T.n_delta[__ffs(lists) - 1] : 0u;
+                uint32_t* K0 = P + (lists ? T.ent_off[__ffs(lists) - 1] : 0u);
+                const uint32_t rest = lists & (lists - 1u);
+                uint32_t wt = 0, tp0 = 0;                                // the window's first token; tokens placed
+                uint32_t wv = lane < n0 ? K0[lane] : 0u;
                 uint32_t run = 0;                                        // occurrences in the blocks already streamed
-                for (uint32_t i0 = 0; i0 < nblk; i0 += 32) {
+                for (uint32_t i0 = 0; i0 < nb; i0 += 32) {
                     const uint32_t bi = i0 + lane;                       // index in streaming (forward-read) order
-                    const bool valid = bi < nblk;
-                    const uint32_t blk = rev ? nblk - 1u - bi : bi;      // block in query order
-                    uint32_t bm = 0;
-                    if (valid) {
+                    const uint32_t blk = rev ? nb - 1u - bi : bi;        // block in query order
+                    uint4 qv[SEL_Q];                                     // (a uint4 wholly past the SEQ is not read)
 #pragma unroll
-                        for (int w = 0; w < 4; w++) {
-                            const uint32_t byte0 = blk * 16 + w * 4;
-                            if (byte0 >= nbytes) continue;
-                            uint32_t word = seqw[blk * 4 + w];
-                            const uint32_t vb = nbytes - byte0;
-                            if (vb < 4) word &= (1u << (8 * vb)) - 1u;
-                            bm |= nib_flags_to_mask(nib_eq_flags(word, 1u << x)) << (8 * w);
+                    for (int h = 0; h < SEL_Q; h++) qv[h] = bi < nb && 16u * (SEL_Q * blk + h) < s_end ? seq4[SEL_Q * blk + h] : make_uint4(0u, 0u, 0u, 0u);
+                    const bool edge = i0 == 0 || i0 + 32 >= nb;          // first / last round: bytes of the grid outside the SEQ
+                    uint32_t cnt = 0;
+#pragma unroll
+                    for (int h = 0; h < SEL_Q; h++) {
+                        uint32_t f[4] = {qv[h].x, qv[h].y, qv[h].z, qv[h].w};
+                        if (edge) {
+#pragma unroll
+                            for (int w = 0; w < 4; w++) {
+                                const uint32_t g = 16u * (SEL_Q * blk + h) + 4u * w;   // grid offset of the word (lanes past the end hold zeros)
+                                if (g < a16) f[w] &= a16 - g >= 4 ? 0u : 0xffffffffu << (8 * (a16 - g));
+                                if (g + 4 > s_end) f[w] &= g >= s_end ? 0u : 0xffffffffu >> (8 * (g + 4 - s_end));
+                            }
                         }
+#pragma unroll
+                        for (int w = 0; w < 4; w++) { f[w] = nib_eq_flags(f[w], 1u << x); cnt += __popc(f[w]); }   // a zero nibble matches no base
+                        s_fq[h][wib][lane] = make_uint4(f[0], f[1], f[2], f[3]);
                     }
-                    const uint32_t cnt = __popc(bm);
                     const uint32_t incl = warp_incl_scan(cnt);
                     s_cb[wib][lane] = run + incl - cnt;
-                    s_bm[wib][lane] = bm;
                     const uint32_t hi = run + __shfl_sync(FULL, incl, 31);      // tokens with index in [run, hi) live here
                     __syncwarp();
-                    uint32_t ls = lists;
+                    auto select = [&](uint32_t k) -> uint32_t {          // forward position of occurrence k, run <= k < hi
+                        uint32_t lo = 0, hb = 32;                        // largest b with s_cb[b] <= k
+#pragma unroll
+                        for (int st = 0; st < 5; st++) { const uint32_t mid = (lo + hb) >> 1; if (s_cb[wib][mid] <= k) lo = mid; else hb = mid; }
+                        const uint32_t c_lo = s_cb[wib][lo];
+                        uint32_t within = k - c_lo;
+                        if (rev) within = (lo < 31 ? s_cb[wib][lo + 1] : hi) - c_lo - 1u - within;   // forward order runs down the query
+                        uint4 fl = s_fq[0][wib][lo];
+                        uint32_t pos = 0;
+#pragma unroll
+                        for (int h = 1; h < SEL_Q; h++) {                // (once found, within stays below the count)
+                            const uint32_t c = __popc(fl.x) + __popc(fl.y) + __popc(fl.z) + __popc(fl.w);
+                            if (within >= c) { within -= c; pos += 32; fl = s_fq[h][wib][lo]; }
+                        }
+                        const uint32_t c0 = __popc(fl.x), c1 = __popc(fl.y), c2 = __popc(fl.z);
+                        uint32_t y = fl.x;
+                        if (within >= c0) {
+                            within -= c0; y = fl.y; pos += 8;
+                            if (within >= c1) {
+                                within -= c1; y = fl.z; pos += 8;
+                                if (within >= c2) { within -= c2; y = fl.w; pos += 8; }
+                            }
+                        }
+                        uint32_t msk = nib_flags_to_mask(y), c;          // the word's 8 bases in base order
+                        c = __popc(msk & 0xfu); if (within >= c) { within -= c; pos += 4; msk >>= 4; }
+                        c = __popc(msk & 0x3u); if (within >= c) { within -= c; pos += 2; msk >>= 2; }
+                        c = msk & 1u;           if (within >= c) { pos += 1; }
+                        const uint32_t bq = rev ? nb - 1u - (i0 + lo) : i0 + lo;
+                        const uint32_t q = bq * (32u * SEL_Q) + pos - 2u * a16;
+                        return rev ? L - 1u - q : q;
+                    };
+                    while (tp0 < n0) {
+                        const uint32_t t = wt + lane;
+                        const bool in = t >= tp0 && t < n0 && wv < hi;
+                        if (in) K0[t] = select(wv);
+                        tp0 += __popc(__ballot_sync(FULL, in));
+                        if (tp0 < wt + 32u) break;                       // the rest of the window lies in later rounds
+                        wt += 32u;
+                        wv = wt + lane < n0 ? K0[wt + lane] : 0u;
+                    }
+                    uint32_t ls = rest;
                     while (ls) {
                         const uint32_t l = __ffs(ls) - 1;
                         ls &= ls - 1;
@@ -778,24 +868,7 @@ __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
                             const uint32_t t = tp + lane;
                             const uint32_t kv = t < n ? Kp[t] : 0xffffffffu;
                             const bool in = t < n && kv < hi;
-                            if (in) {
-                                // largest b with s_cb[b] <= kv
-                                uint32_t lo = 0, hb = 32;
-#pragma unroll
-                                for (int st = 0; st < 5; st++) { const uint32_t mid = (lo + hb) >> 1; if (s_cb[wib][mid] <= kv) lo = mid; else hb = mid; }
-                                uint32_t msk = s_bm[wib][lo];
-                                uint32_t within = kv - s_cb[wib][lo];
-                                if (rev) within = __popc(msk) - 1u - within;          // forward order runs down the query
-                                uint32_t pos = 0, c;
-                                c = __popc(msk & 0xffffu); if (within >= c) { within -= c; pos += 16; msk >>= 16; }
-                                c = __popc(msk & 0xffu);   if (within >= c) { within -= c; pos += 8;  msk >>= 8; }
-                                c = __popc(msk & 0xfu);    if (within >= c) { within -= c; pos += 4;  msk >>= 4; }
-                                c = __popc(msk & 0x3u);    if (within >= c) { within -= c; pos += 2;  msk >>= 2; }
-                                c = msk & 1u;              if (within >= c) { pos += 1; }
-                                const uint32_t bq = rev ? nblk - 1u - (i0 + lo) : i0 + lo;
-                                const uint32_t q = bq * 32 + pos;
-                                Kp[t] = rev ? L - 1u - q : q;
-                            }
+                            if (in) Kp[t] = select(kv);
                             const uint32_t c_in = __popc(__ballot_sync(FULL, in));
                             tp += c_in;
                             if (c_in < 32) break;
@@ -805,15 +878,18 @@ __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
                     }
                     run = hi;
                     __syncwarp();
+                    PCLK_COUNT(8, 1);
                 }
                 if (lane == 0) T.tot[x] = run;
                 // a token left unplaced refers to an occurrence past the end of the read (mod_bam.rs:705-727)
-                uint32_t ls = lists;
+                if (tp0 < n0) err = true;
+                uint32_t ls = rest;
                 while (ls) { const uint32_t l = __ffs(ls) - 1; ls &= ls - 1; if (s_tp[wib][l] < T.n_delta[l]) err = true; }
                 __syncwarp();
             }
         }
         __syncwarp();
+        PCLK(5);
         // '.'/default-mode lists (src/read_cache.rs:122-137, src/mod_bam.rs:1041-1043, 1265-1292)
         bool any_entries = ent > 0;
         uint32_t imp_lists[2][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}};   // lists that infer canonical on (strand, base)
@@ -857,7 +933,9 @@ __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
             }
         }
         __syncwarp();
+        PCLK(6);
     }
+    PCLK_FLUSH;
 }
 
 // Kernel B: per read with mod info: CIGAR prefix, then every list entry -> merged probabilities -> collapse ->
