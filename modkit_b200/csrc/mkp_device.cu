@@ -8,11 +8,13 @@
 
 #include <algorithm>
 #include <cctype>
+#include <cstddef>
 #include <cstdlib>
 #include <cstdio>
 #include <cstring>
 #include <string>
 #include <thread>
+#include <utility>
 #include <vector>
 
 #include "mkp_kernels.cuh"
@@ -27,6 +29,10 @@ namespace {
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
     cudaError_t ensure(size_t bytes) {
         if (bytes <= cap) return cudaSuccess;
         if (p) cudaFree(p);
@@ -38,7 +44,6 @@ struct DevBuf {
         if (e == cudaSuccess) cap = want;
         return e;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
     template <class T> T* as() const { return (T*)p; }
 };
 
@@ -73,7 +78,7 @@ struct mkp_ctx {
     uint64_t launches = 0;       // kernels launched by this context (mkp_kernel_launches)
     double pass_prof[4] = {0, 0, 0, 0};          // same for the pileup pass: buffers, launches, wait, calls
     double slice_prof[6] = {0, 0, 0, 0, 0, 0};   // MKP_TRACE_SLICE=1: host seconds in the phases of mkp_bam_chunk, printed by mkp_destroy
-    // fused pass (chunks with focus bitmaps): tile table, rank of the focus set (built at upload), capacities
+    // focus-rank pass (chunks with focus bitmaps): tile table, rank of the focus set (built at upload), capacities
     DevBuf d_pscr, d_inftab, d_tiles, d_order;
     bool order_ready = false;
     uint32_t n_tiles = 0;
@@ -92,17 +97,39 @@ struct mkp_ctx {
     mkp_row* h_rows_pinned = nullptr;
     size_t h_rows_pinned_cap = 0;
     // pileup-hemi pass: interval starts, its own hot bitmap (k_resolve's marks) and focus rank (d_hot / d_hot_prefix hold the
-    // rank the fused pileup pass builds once per chunk), rows (device, host)
+    // rank the focus-rank pileup pass builds once per chunk), rows (device, host)
     DevBuf d_iv_start, d_hemi_hot, d_hemi_prefix, d_hemi_rows;
     size_t n_hemi_rows = 0;
     std::vector<mkp_hemi_row> h_hemi_rows;
 };
 
-// d_small layout (u64 words): [0..31] states, [32] total_calls, [33] hist_inexact ; u32 view from byte 34*8: n_states, err, n_hot, n_rows
-static constexpr size_t SMALL_BYTES = 34 * 8 + 16 * 4;
+// d_small: the words the kernels of a pass share and the host reads back. A pass clears all of it (clear_scratch); the ingest
+// and mkp_bam_tags zero only their own words.
+struct PassScratch {
+    unsigned long long states[MAX_STATES];   // (base << 32 | code) of every state id, ~0 = unused
+    unsigned long long total_calls;
+    unsigned long long hist_inexact;
+    uint32_t n_states, err;                  // distinct states seen, MKP_DERR_* bits
+    uint32_t n_hot, n_rows;                  // rank total (counter slots), row-count scan total
+    uint32_t work[6];                        // ChunkDev::work (CountDev::work and HemiDev::work are work + 2)
+    uint32_t ingest_status;                  // k_inflate / k_walk error word
+    uint32_t n_records;                      // ingest: record-count scan total
+    uint32_t read_counter;                   // FusedDev::read_counter
+    uint32_t tile_counter;                   // TileDev::tile_counter
+    uint32_t tag_overflow;                   // k_tag_values
+};
+static_assert(sizeof(PassScratch) == 336 && offsetof(PassScratch, n_states) == 272 && offsetof(PassScratch, work) == 288 &&
+              offsetof(PassScratch, read_counter) == 320 && offsetof(PassScratch, tag_overflow) == 328, "d_small layout");
 
 static int fail(mkp_ctx* c, const std::string& m, int code = -1) { if (c) c->err = m; return code; }
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail(ctx, std::string(#call) + ": " + cudaGetErrorString(e_)); } while (0)
+
+// Every kernel launch of this file goes through here, so mkp_kernel_launches counts exactly the launches issued.
+template <class... P, class... A>
+static void launch(mkp_ctx* ctx, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
+    ctx->launches += 1;
+    kernel<<<grid, block, smem, st>>>(std::forward<A>(args)...);
+}
 
 extern "C" {
 
@@ -171,20 +198,13 @@ void mkp_destroy(mkp_ctx* ctx) {
     if (getenv("MKP_TRACE_SLICE")) fprintf(stderr, "[mkp] slice phases (s): buffers %.4f plan+scan %.4f heap alloc %.4f copy+focus %.4f finish_upload %.4f calls %.0f\n",
                                            ctx->slice_prof[0], ctx->slice_prof[1], ctx->slice_prof[2], ctx->slice_prof[3], ctx->slice_prof[4], ctx->slice_prof[5]);
     if (getenv("MKP_TRACE_SLICE")) fprintf(stderr, "[mkp] pass phases (s): buffers %.4f launches %.4f wait %.4f calls %.0f\n", ctx->pass_prof[0], ctx->pass_prof[1], ctx->pass_prof[2], ctx->pass_prof[3]);
-    DevBuf* bufs[] = {&ctx->d_hdrs, &ctx->d_heap, &ctx->d_entry_off, &ctx->d_focus_pos, &ctx->d_focus_neg, &ctx->d_rl, &ctx->d_meta, &ctx->d_P,
-                      &ctx->d_calls, &ctx->d_hot, &ctx->d_hot_prefix, &ctx->d_wrec, &ctx->d_block_sums, &ctx->d_small, &ctx->d_scr_cq, &ctx->d_scr_cr, &ctx->d_slow,
-                      &ctx->d_obs_word, &ctx->d_slots, &ctx->d_row_counts, &ctx->d_row_prefix, &ctx->d_rows, &ctx->d_hist, &ctx->d_take,
-                      &ctx->d_file, &ctx->d_members, &ctx->d_bam, &ctx->d_seeds, &ctx->d_seg_counts, &ctx->d_seg_base, &ctx->d_recs, &ctx->d_ids, &ctx->d_plan,
-                      &ctx->d_need, &ctx->d_totals, &ctx->d_slab_work, &ctx->d_pscr, &ctx->d_inftab, &ctx->d_tiles, &ctx->d_order,
-                      &ctx->d_iv_start, &ctx->d_hemi_hot, &ctx->d_hemi_prefix, &ctx->d_hemi_rows};
-    for (auto* b : bufs) b->release();
     if (ctx->h_rows_pinned) cudaFreeHost(ctx->h_rows_pinned);
     for (int i = 0; i < ctx->n_pin; i++) { cudaFreeHost(ctx->pin[i]); cudaEventDestroy(ctx->pin_ev[i]); }
     for (auto& e : ctx->ev) cudaEventDestroy(e);
     cudaEventDestroy(ctx->ev_fork); cudaEventDestroy(ctx->ev_join);
     cudaStreamDestroy(ctx->stream2);
     cudaStreamDestroy(ctx->stream);
-    delete ctx;
+    delete ctx;                 // frees the device buffers, on ctx->device
 }
 
 const char* mkp_last_error(const mkp_ctx* ctx) { return ctx ? ctx->err.c_str() : "null context"; }
@@ -253,7 +273,7 @@ static int decode_grid(const mkp_ctx* ctx, uint32_t n_reads) {
     return std::max(1, std::min(blocks, need));
 }
 
-static int prepare_decode(mkp_ctx* ctx, ChunkDev* C, int grid) {
+static int prepare_decode(mkp_ctx* ctx, ChunkDev* C, int grid, uint32_t mode) {
     const size_t nwarps = (size_t)grid * 4;
     CK(ctx->d_meta.ensure(std::max<size_t>(1, ctx->n_reads) * sizeof(ReadMeta)));
     CK(ctx->d_rl.ensure(std::max<size_t>(1, ctx->n_reads) * sizeof(ReadLists)));
@@ -262,7 +282,7 @@ static int prepare_decode(mkp_ctx* ctx, ChunkDev* C, int grid) {
     CK(ctx->d_hot.ensure((size_t)ctx->n_words * 8 + 4));
     CK(ctx->d_hot_prefix.ensure((size_t)ctx->n_words * 8 + 4));
     CK(ctx->d_wrec.ensure((size_t)ctx->n_words * 16 + 16));
-    CK(ctx->d_small.ensure(SMALL_BYTES));
+    CK(ctx->d_small.ensure(sizeof(PassScratch)));
     CK(ctx->d_scr_cq.ensure(nwarps * ((size_t)ctx->max_ncigar + 4) * 4));
     CK(ctx->d_scr_cr.ensure(nwarps * ((size_t)ctx->max_ncigar + 4) * 4));
     memset(C, 0, sizeof *C);
@@ -272,17 +292,16 @@ static int prepare_decode(mkp_ctx* ctx, ChunkDev* C, int grid) {
     C->focus_neg = ctx->have_focus ? ctx->d_focus_neg.as<uint32_t>() : nullptr;
     C->meta = ctx->d_meta.as<ReadMeta>(); C->P = ctx->d_P.as<uint32_t>(); C->calls = ctx->d_calls.as<uint2>();
     C->hot = ctx->d_hot.as<uint32_t>(); C->hot_prefix = ctx->d_hot_prefix.as<uint32_t>();
-    C->states = ctx->d_small.as<unsigned long long>();
-    C->total_calls = C->states + 32;
-    C->hist_inexact = C->states + 33;
-    uint32_t* u = (uint32_t*)(ctx->d_small.as<uint8_t>() + 34 * 8);
-    C->n_states = u; C->err = u + 1; C->work = u + 4;
+    PassScratch* const s = ctx->d_small.as<PassScratch>();
+    C->states = s->states; C->total_calls = &s->total_calls; C->hist_inexact = &s->hist_inexact;
+    C->n_states = &s->n_states; C->err = &s->err; C->work = s->work;
     C->scr_cq = ctx->d_scr_cq.as<uint32_t>(); C->scr_cr = ctx->d_scr_cr.as<uint32_t>();
     C->max_ncigar = ctx->max_ncigar; C->max_blocks = ctx->max_blocks;
     C->rl = ctx->d_rl.as<ReadLists>();
     CK(ctx->d_slow.ensure((size_t)ctx->n_reads * 4 + 4));
     C->slow_list = ctx->d_slow.as<uint32_t>();
     C->order = ctx->order_ready ? ctx->d_order.as<uint32_t>() : nullptr;
+    C->mode = mode;
     return 0;
 }
 
@@ -294,8 +313,122 @@ static std::string derr_text(uint32_t e) {
     return s;
 }
 
+// ---- steps shared by the passes ------------------------------------------------------------------------------------------
+
+// 0xff fill of the state registry (~0 = unused id), zero fill of the rest of the scratch block
+static int clear_scratch(mkp_ctx* ctx) {
+    PassScratch* const s = ctx->d_small.as<PassScratch>();
+    CK(cudaMemsetAsync(s->states, 0xff, sizeof s->states, ctx->stream));
+    CK(cudaMemsetAsync(&s->total_calls, 0, sizeof(PassScratch) - offsetof(PassScratch, total_calls), ctx->stream));
+    return 0;
+}
+
+// the scratch block, once the work enqueued on the stream is done
+static int read_scratch(mkp_ctx* ctx, PassScratch* h) {
+    CK(cudaMemcpyAsync(h, ctx->d_small.p, sizeof *h, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// read_scratch; a decode error of the device fails the pass, with stats->device_error set
+static int finish_status(mkp_ctx* ctx, mkp_stats* stats, PassScratch* h) {
+    if (int rc = read_scratch(ctx, h)) return rc;
+    if (!h->err) return 0;
+    if (stats) { memset(stats, 0, sizeof *stats); stats->device_error = h->err; }
+    return fail(ctx, "device decode error: " + derr_text(h->err), -10);
+}
+
+// k_parse, then k_resolve: the fast instantiation over every read, then the generic one over the reads it left. ev[1] marks the
+// end of the parse, ev[2] the end of the resolve. List mode (C.list_mode == 1: the reads k_pileup_fused left, all of which need
+// the generic resolve) runs no fast resolve and records no event: its caller times it with the counting kernels.
+static int decode(mkp_ctx* ctx, const ChunkDev& C, int grid) {
+    cudaStream_t st = ctx->stream;
+    const bool hist = C.mode == MODE_HIST, list = C.list_mode == 1;
+    if (C.n_reads) launch(ctx, k_parse, grid, 128, 0, st, C);
+    if (!list) CK(cudaEventRecord(ctx->ev[1], st));
+    if (C.n_reads && !list) launch(ctx, hist ? k_resolve<MODE_HIST, true> : k_resolve<MODE_PILEUP, true>, grid, 128, 0, st, C);
+    if (C.n_reads) launch(ctx, hist ? k_resolve<MODE_HIST, false> : k_resolve<MODE_PILEUP, false>, grid, 128, 0, st, C);
+    if (!list) CK(cudaEventRecord(ctx->ev[2], st));
+    return 0;
+}
+
+// rank of the set bits of bits[0 .. n): prefix[i] = bits set before word i, *total = all of them. With focus_pos / focus_neg,
+// `bits` is the [2][n / 2] per-strand pair and first loses its marks outside the strand's focus set.
+static int rank_bits(mkp_ctx* ctx, uint32_t* bits, uint32_t n, const uint32_t* focus_pos, const uint32_t* focus_neg, uint32_t* prefix,
+                     uint32_t* total) {
+    const uint32_t n_blk = (n + 1023) / 1024;
+    CK(ctx->d_block_sums.ensure((size_t)n_blk * 4 + 4));
+    uint32_t* const sums = ctx->d_block_sums.as<uint32_t>();
+    launch(ctx, k_block_popc, n_blk, 1024, 0, ctx->stream, bits, n, sums, focus_pos, focus_neg);
+    launch(ctx, k_scan_blocks, 1, 1024, 0, ctx->stream, sums, n_blk, total);
+    launch(ctx, k_word_prefix, n_blk, 1024, 0, ctx->stream, bits, n, sums, prefix);
+    return 0;
+}
+
+// exclusive prefix sum of values[0 .. n) into prefix, and the sum into *total
+static int exclusive_scan_u32(mkp_ctx* ctx, const uint32_t* values, uint32_t n, uint32_t* prefix, uint32_t* total) {
+    const uint32_t n_blk = (n + 1023) / 1024;
+    CK(ctx->d_block_sums.ensure((size_t)n_blk * 4 + 4));
+    uint32_t* const sums = ctx->d_block_sums.as<uint32_t>();
+    launch(ctx, k_block_sum, n_blk, 1024, 0, ctx->stream, values, n, sums);
+    launch(ctx, k_scan_blocks, 1, 1024, 0, ctx->stream, sums, n_blk, total);
+    launch(ctx, k_value_prefix, n_blk, 1024, 0, ctx->stream, values, n, sums, prefix);
+    return 0;
+}
+
+// the counting kernels over the pileup pass's slots (`stride` words, n_states states each) and word records
+static CountDev count_dev(const mkp_ctx* ctx, const ChunkDev& C, uint32_t stride, uint32_t n_states) {
+    CountDev D;
+    D.hdrs = C.hdrs; D.heap = C.heap; D.meta = C.meta; D.calls = C.calls; D.n_reads = C.n_reads; D.cs = C.cs; D.ce = C.ce;
+    D.rec = ctx->d_wrec.as<uint4>();
+    D.slots = ctx->d_slots.as<uint32_t>(); D.stride = stride; D.n_states = n_states; D.n_words = ctx->n_words;
+    D.obs_word = ctx->d_obs_word.as<uint32_t>(); D.work = C.work + 2;
+    D.list = nullptr; D.list_count = nullptr;
+    D.order = nullptr;          // (the counting kernels keep the coordinate order: neighbouring reads update neighbouring slots)
+    return D;
+}
+
+// k_count_calls on stream2 beside k_count_bases: the two only meet in commutative atomics on the slots, and both are
+// latency-bound at 32 registers, so they co-reside on the SMs
+static int count_side_by_side(mkp_ctx* ctx, const CountDev& D) {
+    const int g2 = std::max(1, std::min(ctx->sm_count * 8, (int)((D.n_reads + 7) / 8)));
+    CK(cudaEventRecord(ctx->ev_fork, ctx->stream));
+    CK(cudaStreamWaitEvent(ctx->stream2, ctx->ev_fork, 0));
+    launch(ctx, k_count_calls, g2, 256, 0, ctx->stream2, D);
+    CK(cudaEventRecord(ctx->ev_join, ctx->stream2));
+    launch(ctx, k_count_bases, g2, 256, 0, ctx->stream, D);
+    CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
+    return 0;
+}
+
+// the row kernels over the same slots, emitting into d_rows as it is now
+static RowDev row_dev(const mkp_ctx* ctx, const ChunkDev& C, uint32_t stride, uint32_t n_states) {
+    RowDev R;
+    R.rec = ctx->d_wrec.as<uint4>(); R.n_words = ctx->n_words; R.cs = C.cs; R.ce = C.ce;
+    R.slots = ctx->d_slots.as<uint32_t>(); R.stride = stride; R.n_states = n_states; R.states = C.states; R.numeric_mode = ctx->params.numeric_mode;
+    R.obs_word = ctx->d_obs_word.as<uint32_t>();
+    R.row_counts = ctx->d_row_counts.as<uint32_t>(); R.row_prefix = ctx->d_row_prefix.as<uint32_t>();
+    R.rows = ctx->d_rows.as<mkp_row>(); R.rows_cap = (uint32_t)std::min<size_t>(0xffffffffu, ctx->d_rows.cap / sizeof(mkp_row));
+    return R;
+}
+
+// mkp_stats::kernel_ms from the events of a pass: 0 start | 1 parsed | 2 resolved | 3 ranked | 4 counting starts | 6 counted |
+// 7 rows counted and scanned | 8 emit starts | 9 end. Every pass: [0] parse, [1] resolve, [4] counters, [5] rows (count, scan,
+// emit), [7] total. The focus-rank pass (`ranked` false) has no rank and no host sync; under MKP_FUSED / MKP_TILE its [0] is the
+// fused kernel and [1] the generic kernels, counting included, over the reads it left. The hot-mark and hemi passes add [2] rank
+// and [6] host syncs and allocations. [3] stays 0 (k_count_calls runs beside k_count_bases, inside [4]).
+static void pass_ms(const mkp_ctx* ctx, bool ranked, float* ms) {
+    auto el = [&](int a, int b) { float t = 0; cudaEventElapsedTime(&t, ctx->ev[a], ctx->ev[b]); return t; };
+    ms[0] = el(0, 1); ms[1] = el(1, 2); ms[7] = el(0, 9);
+    if (!ranked) { ms[4] = el(2, 6); ms[5] = el(6, 9); return; }
+    ms[2] = el(2, 3); ms[4] = el(4, 6); ms[5] = el(6, 7) + el(8, 9); ms[6] = el(3, 4) + el(7, 8);
+}
+
+// ---- the passes ------------------------------------------------------------------------------------------------------------
+
 // Chunks with focus bitmaps: the positions that can produce rows are known at upload, so the rank structure (counter slot of
-// every focus position) and the tile table of the fused pass are built here, once per chunk, not once per pass.
+// every focus position) and the tile table of k_pileup_tile are built here, once per chunk, not once per pass.
 static int finish_upload(mkp_ctx* ctx) {
     ctx->focus_ready = false;
     ctx->order_ready = false;
@@ -305,53 +438,46 @@ static int finish_upload(mkp_ctx* ctx) {
         uint32_t* hist = ctx->d_order.as<uint32_t>() + ctx->n_reads;
         CK(cudaMemsetAsync(hist, 0, 32 * 4, st));
         const int g = (int)((ctx->n_reads + 255) / 256);
-        ctx->launches += 3;
-        k_order_hist<<<g, 256, 0, st>>>(ctx->d_hdrs.as<mkp_read_hdr>(), ctx->n_reads, hist);
-        k_order_scan<<<1, 1, 0, st>>>(hist);
-        k_order_scatter<<<g, 256, 0, st>>>(ctx->d_hdrs.as<mkp_read_hdr>(), ctx->n_reads, hist, ctx->d_order.as<uint32_t>());
+        launch(ctx, k_order_hist, g, 256, 0, st, ctx->d_hdrs.as<mkp_read_hdr>(), ctx->n_reads, hist);
+        launch(ctx, k_order_scan, 1, 1, 0, st, hist);
+        launch(ctx, k_order_scatter, g, 256, 0, st, ctx->d_hdrs.as<mkp_read_hdr>(), ctx->n_reads, hist, ctx->d_order.as<uint32_t>());
         ctx->order_ready = true;
     }
     if (!ctx->have_focus) { CK(cudaStreamSynchronize(st)); CK(cudaGetLastError()); return 0; }
     // counter slot of every (focus position, strand): its rank in the [2][n_words] pair (focus_pos, focus_neg)
     const uint32_t n_words = ctx->n_words;
-    const uint32_t n_blk = (2 * n_words + 1023) / 1024;
     CK(ctx->d_hot.ensure((size_t)n_words * 8 + 4));
     CK(ctx->d_hot_prefix.ensure((size_t)n_words * 8 + 4));
     CK(ctx->d_wrec.ensure((size_t)n_words * 16 + 16));
-    CK(ctx->d_block_sums.ensure((size_t)n_blk * 4 + 4));
-    CK(ctx->d_small.ensure(SMALL_BYTES));
-    uint32_t* u = (uint32_t*)(ctx->d_small.as<uint8_t>() + 34 * 8);
-    CK(cudaMemcpyAsync(ctx->d_hot.p, ctx->d_focus_pos.p, (size_t)n_words * 4, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(ctx->d_hot.as<uint32_t>() + n_words, ctx->d_focus_neg.p, (size_t)n_words * 4, cudaMemcpyDeviceToDevice, st));
-    ctx->launches += 4;
-    k_block_popc<<<n_blk, 1024, 0, st>>>(ctx->d_hot.as<uint32_t>(), 2 * n_words, ctx->d_block_sums.as<uint32_t>(), nullptr, nullptr);
-    k_scan_blocks<<<1, 1024, 0, st>>>(ctx->d_block_sums.as<uint32_t>(), n_blk, u + 2);
-    k_word_prefix<<<n_blk, 1024, 0, st>>>(ctx->d_hot.as<uint32_t>(), 2 * n_words, ctx->d_block_sums.as<uint32_t>(), ctx->d_hot_prefix.as<uint32_t>());
-    k_word_record<<<(n_words + 255) / 256, 256, 0, st>>>(ctx->d_hot.as<uint32_t>(), ctx->d_hot_prefix.as<uint32_t>(), n_words, ctx->d_wrec.as<uint4>());
-    uint32_t n_hot = 0;
-    CK(cudaMemcpyAsync(&n_hot, u + 2, 4, cudaMemcpyDeviceToHost, st));
+    CK(ctx->d_small.ensure(sizeof(PassScratch)));
+    uint32_t* const hot = ctx->d_hot.as<uint32_t>();
+    uint32_t* const hot_prefix = ctx->d_hot_prefix.as<uint32_t>();
+    CK(cudaMemcpyAsync(hot, ctx->d_focus_pos.p, (size_t)n_words * 4, cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(hot + n_words, ctx->d_focus_neg.p, (size_t)n_words * 4, cudaMemcpyDeviceToDevice, st));
+    if (int rc = rank_bits(ctx, hot, 2 * n_words, nullptr, nullptr, hot_prefix, &ctx->d_small.as<PassScratch>()->n_hot)) return rc;
+    launch(ctx, k_word_record, (n_words + 255) / 256, 256, 0, st, hot, hot_prefix, n_words, ctx->d_wrec.as<uint4>());
     ctx->n_tiles = ctx->n_reads ? (uint32_t)((ctx->heap_bytes + TL_WIN - 1) / TL_WIN) : 0;
     if (ctx->n_tiles == 0 && ctx->n_reads) ctx->n_tiles = 1;
     CK(ctx->d_tiles.ensure(((size_t)ctx->n_tiles + 1) * sizeof(TileInfo)));
-    ctx->launches += 1;
-    k_tiles<<<(ctx->n_tiles + 1 + 255) / 256, 256, 0, st>>>(ctx->d_hdrs.as<mkp_read_hdr>(), ctx->n_reads, ctx->heap_bytes, ctx->d_tiles.as<TileInfo>(), ctx->n_tiles);
-    CK(cudaStreamSynchronize(st));
-    CK(cudaGetLastError());
-    ctx->n_hot = n_hot;
+    launch(ctx, k_tiles, (ctx->n_tiles + 1 + 255) / 256, 256, 0, st, ctx->d_hdrs.as<mkp_read_hdr>(), ctx->n_reads, ctx->heap_bytes,
+           ctx->d_tiles.as<TileInfo>(), ctx->n_tiles);
+    PassScratch h;
+    if (int rc = read_scratch(ctx, &h)) return rc;
+    ctx->n_hot = h.n_hot;
     ctx->focus_ready = true;
     return 0;
 }
 
-// The pass for chunks with focus bitmaps: k_pileup_fused, the generic kernels over the reads it left, the row kernels. Everything
-// is enqueued at once; the host reads the counters once, at the end (capacities that turn out too small - distinct
-// (base, code) states per slot, rows - grow and the affected part runs again).
-static int pileup_fused(mkp_ctx* ctx, mkp_stats* stats) {
+// The focus-rank pass, for chunks with focus bitmaps: the counter slots are the rank built at upload, so everything is enqueued
+// at once and the host reads the counters once, at the end (capacities that turn out too small - distinct (base, code) states
+// per slot, rows - grow and the affected part runs again). It runs the per-stage kernels over every read, unless MKP_FUSED=1 or
+// MKP_TILE=1 selects a fused kernel that counts most reads in one traversal and leaves the rest to the generic kernels.
+static int pileup_focus(mkp_ctx* ctx, mkp_stats* stats) {
     cudaStream_t st = ctx->stream;
     auto now = [] { return std::chrono::steady_clock::now(); };
     auto since = [&](std::chrono::steady_clock::time_point t) { return std::chrono::duration<double>(now() - t).count(); };
     auto tp = now();
     const uint32_t n_words = ctx->n_words, n_hot = ctx->n_hot;
-    const uint32_t n_blk = (n_words + 1023) / 1024;
     ChunkDev C;
     // MKP_FUSED=1: the TMA-staged single-traversal kernel (k_pileup_fused); default: the per-stage kernels (see DESIGN.md 4:
     // the pass is bound by instruction issue, and the per-stage kernels keep 2-3x more warps per SM in flight)
@@ -360,8 +486,7 @@ static int pileup_fused(mkp_ctx* ctx, mkp_stats* stats) {
     const bool use_tile = tl && tl[0] == '1';                  // k_pileup_tile: CTA-cooperative phases over TMA-staged tiles
     const bool use_fused = use_tile || (fz && fz[0] == '1');
     const int g_slow = use_fused ? std::max(1, std::min(ctx->sm_count * 2, (int)((ctx->n_reads + 3) / 4))) : decode_grid(ctx, ctx->n_reads);
-    if (int rc = prepare_decode(ctx, &C, g_slow)) return rc;
-    CK(ctx->d_block_sums.ensure((size_t)n_blk * 4 + 4));
+    if (int rc = prepare_decode(ctx, &C, g_slow, MODE_PILEUP)) return rc;
     CK(ctx->d_row_counts.ensure((size_t)n_words * 4 + 4));
     CK(ctx->d_row_prefix.ensure((size_t)n_words * 4 + 4));
     CK(ctx->d_obs_word.ensure((size_t)n_words * 8 + 8));
@@ -372,11 +497,8 @@ static int pileup_fused(mkp_ctx* ctx, mkp_stats* stats) {
         CK(cudaFuncSetAttribute(k_pileup_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FzShared)));
         ctx->fused_attr_set = true;
     }
-    uint32_t* u = (uint32_t*)(ctx->d_small.as<uint8_t>() + 34 * 8);   // n_states, err, n_hot, n_rows, work[0..5] = u+4.., tile counter u+12
-    uint32_t h_small[4] = {0, 0, 0, 0};
-    unsigned long long h_calls = 0;
-    uint32_t h_slow = 0;
-    bool fused_ran = false;
+    PassScratch* const s = ctx->d_small.as<PassScratch>();
+    PassScratch h;
     for (int attempt = 0;; attempt++) {
         const uint32_t S_cap = ctx->state_cap;
         const uint32_t stride = SL_MOD + S_cap;
@@ -384,230 +506,142 @@ static int pileup_fused(mkp_ctx* ctx, mkp_stats* stats) {
         if (!ctx->d_rows.p) CK(ctx->d_rows.ensure(std::max<size_t>(1024, (size_t)n_hot * 3) * sizeof(mkp_row)));
         ctx->pass_prof[0] += since(tp); tp = now();
         CK(cudaEventRecord(ctx->ev[0], st));
-        CK(cudaMemsetAsync(ctx->d_small.p, 0xff, 32 * 8, st));
-        CK(cudaMemsetAsync(ctx->d_small.as<uint8_t>() + 32 * 8, 0, SMALL_BYTES - 32 * 8, st));
+        if (int rc = clear_scratch(ctx)) return rc;
         CK(cudaMemsetAsync(ctx->d_slots.p, 0, (size_t)n_hot * stride * 4, st));
         CK(cudaMemsetAsync(ctx->d_obs_word.p, 0, (size_t)n_words * 8, st));
-        FusedDev F;
-        memset(&F, 0, sizeof F);
-        F.hdrs = C.hdrs; F.heap = C.heap; F.n_reads = C.n_reads; F.cs = C.cs; F.ce = C.ce;
-        F.read_counter = u + 12;
-        F.rec = ctx->d_wrec.as<uint4>();
-        F.slots = ctx->d_slots.as<uint32_t>(); F.stride = stride; F.n_states = S_cap; F.n_words = n_words;
-        F.obs_word = ctx->d_obs_word.as<uint32_t>();
-        F.states = C.states; F.n_states_seen = C.n_states; F.err = C.err;
-        F.slow_list = C.slow_list; F.slow_count = C.work + 4; F.total_calls = C.total_calls;
-        F.p_scratch = ctx->d_pscr.as<uint32_t>(); F.p_stride = ctx->p_stride;
-        C.mode = MODE_PILEUP;
-        CountDev D;
-        D.hdrs = C.hdrs; D.heap = C.heap; D.meta = C.meta; D.calls = C.calls; D.n_reads = C.n_reads; D.cs = C.cs; D.ce = C.ce;
-        D.rec = F.rec;
-        D.slots = F.slots; D.stride = stride; D.n_states = S_cap; D.n_words = n_words; D.obs_word = F.obs_word; D.work = u + 6;
-        D.order = nullptr;          // (the counting kernels keep the coordinate order: neighbouring reads update neighbouring slots)
+        CountDev D = count_dev(ctx, C, stride, S_cap);
         if (use_fused) {
+            FusedDev F;
+            memset(&F, 0, sizeof F);
+            F.hdrs = C.hdrs; F.heap = C.heap; F.n_reads = C.n_reads; F.cs = C.cs; F.ce = C.ce;
+            F.read_counter = &s->read_counter;
+            F.rec = D.rec;
+            F.slots = D.slots; F.stride = stride; F.n_states = S_cap; F.n_words = n_words;
+            F.obs_word = D.obs_word;
+            F.states = C.states; F.n_states_seen = C.n_states; F.err = C.err;
+            F.slow_list = C.slow_list; F.slow_count = &s->work[4]; F.total_calls = C.total_calls;
+            F.p_scratch = ctx->d_pscr.as<uint32_t>(); F.p_stride = ctx->p_stride;
             if (ctx->n_reads && use_tile) {
                 if (!ctx->tile_attr_set) { CK(cudaFuncSetAttribute(k_pileup_tile, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TlShared))); ctx->tile_attr_set = true; }
                 TileDev Tl;
-                Tl.F = F; Tl.tiles = ctx->d_tiles.as<TileInfo>(); Tl.n_tiles = ctx->n_tiles; Tl.tile_counter = u + 13;
-                ctx->launches += 1;
-                k_pileup_tile<<<grid, TL_THREADS, sizeof(TlShared), st>>>(Tl);
-            } else if (ctx->n_reads) { ctx->launches += 1; k_pileup_fused<<<grid, FZ_THREADS, sizeof(FzShared), st>>>(F); }
+                Tl.F = F; Tl.tiles = ctx->d_tiles.as<TileInfo>(); Tl.n_tiles = ctx->n_tiles; Tl.tile_counter = &s->tile_counter;
+                launch(ctx, k_pileup_tile, grid, TL_THREADS, sizeof(TlShared), st, Tl);
+            } else if (ctx->n_reads) launch(ctx, k_pileup_fused, grid, FZ_THREADS, sizeof(FzShared), st, F);
             CK(cudaEventRecord(ctx->ev[1], st));
             // the reads the fused kernel left to the generic path (list mode); both add into the same slots
             C.list_mode = 1;
-            D.list = C.slow_list; D.list_count = C.work + 4;
+            D.list = C.slow_list; D.list_count = &s->work[4];
+            if (int rc = decode(ctx, C, g_slow)) return rc;
             if (ctx->n_reads) {
-                ctx->launches += 4;
-                k_parse<<<g_slow, 128, 0, st>>>(C);
-                k_resolve<MODE_PILEUP, false><<<g_slow, 128, 0, st>>>(C);
                 const int g2 = std::max(1, std::min(ctx->sm_count * 2, (int)((ctx->n_reads + 7) / 8)));
-                k_count_calls<<<g2, 256, 0, st>>>(D);
-                k_count_bases<<<g2, 256, 0, st>>>(D);
+                launch(ctx, k_count_calls, g2, 256, 0, st, D);
+                launch(ctx, k_count_bases, g2, 256, 0, st, D);
             }
             CK(cudaEventRecord(ctx->ev[2], st));
-            CK(cudaEventRecord(ctx->ev[4], st));
         } else {
             // the per-stage kernels at full occupancy (every read), counters addressed by the rank of the focus bit: no hot
             // marks, no rank pass, no host round trip between the stages
             C.list_mode = 2;
-            D.list = nullptr; D.list_count = nullptr;
-            const int gd = decode_grid(ctx, ctx->n_reads);
+            if (int rc = decode(ctx, C, decode_grid(ctx, ctx->n_reads))) return rc;
             if (ctx->n_reads) {
-                ctx->launches += 5;
-                k_parse<<<gd, 128, 0, st>>>(C);
-                CK(cudaEventRecord(ctx->ev[1], st));
-                k_resolve<MODE_PILEUP, true><<<gd, 128, 0, st>>>(C);
-                k_resolve<MODE_PILEUP, false><<<gd, 128, 0, st>>>(C);
-                CK(cudaEventRecord(ctx->ev[2], st));
-                const int g2 = std::max(1, std::min(ctx->sm_count * 8, (int)((ctx->n_reads + 7) / 8)));
-                CK(cudaEventRecord(ctx->ev_fork, st));
-                CK(cudaStreamWaitEvent(ctx->stream2, ctx->ev_fork, 0));
-                k_count_calls<<<g2, 256, 0, ctx->stream2>>>(D);
-                CK(cudaEventRecord(ctx->ev_join, ctx->stream2));
-                k_count_bases<<<g2, 256, 0, st>>>(D);
-                CK(cudaStreamWaitEvent(st, ctx->ev_join, 0));
-            } else { CK(cudaEventRecord(ctx->ev[1], st)); CK(cudaEventRecord(ctx->ev[2], st)); }
-            CK(cudaEventRecord(ctx->ev[4], st));
+                if (int rc = count_side_by_side(ctx, D)) return rc;
+            }
         }
-        RowDev R;
-        R.rec = F.rec; R.n_words = n_words; R.cs = C.cs; R.ce = C.ce;
-        R.slots = F.slots; R.stride = stride; R.n_states = S_cap; R.states = C.states; R.numeric_mode = ctx->params.numeric_mode;
-        R.obs_word = F.obs_word;
-        R.row_counts = ctx->d_row_counts.as<uint32_t>(); R.row_prefix = ctx->d_row_prefix.as<uint32_t>();
-        R.rows = ctx->d_rows.as<mkp_row>(); R.rows_cap = (uint32_t)std::min<size_t>(0xffffffffu, ctx->d_rows.cap / sizeof(mkp_row));
+        CK(cudaEventRecord(ctx->ev[6], st));
+        RowDev R = row_dev(ctx, C, stride, S_cap);
         const int rg = (n_words + 255) / 256;
-        ctx->launches += 5;
-        k_rows<false><<<rg, 256, 0, st>>>(R);
-        k_block_sum<<<n_blk, 1024, 0, st>>>(R.row_counts, n_words, ctx->d_block_sums.as<uint32_t>());
-        k_scan_blocks<<<1, 1024, 0, st>>>(ctx->d_block_sums.as<uint32_t>(), n_blk, u + 3);
-        k_value_prefix<<<n_blk, 1024, 0, st>>>(R.row_counts, n_words, ctx->d_block_sums.as<uint32_t>(), ctx->d_row_prefix.as<uint32_t>());
-        k_rows<true><<<rg, 256, 0, st>>>(R);
-        CK(cudaEventRecord(ctx->ev[3], st));
-        fused_ran = use_fused;
-        CK(cudaMemcpyAsync(h_small, u, 16, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(&h_slow, u + 8, 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(&h_calls, C.total_calls, 8, cudaMemcpyDeviceToHost, st));
+        launch(ctx, k_rows<false>, rg, 256, 0, st, R);
+        if (int rc = exclusive_scan_u32(ctx, R.row_counts, n_words, ctx->d_row_prefix.as<uint32_t>(), &s->n_rows)) return rc;
+        launch(ctx, k_rows<true>, rg, 256, 0, st, R);
+        CK(cudaEventRecord(ctx->ev[9], st));
         ctx->pass_prof[1] += since(tp); tp = now();
-        CK(cudaStreamSynchronize(st));
-        CK(cudaGetLastError());
+        const int rc = finish_status(ctx, stats, &h);
         ctx->pass_prof[2] += since(tp); tp = now();
-        if (h_small[1]) {
-            if (stats) { memset(stats, 0, sizeof *stats); stats->device_error = h_small[1]; }
-            return fail(ctx, "device decode error: " + derr_text(h_small[1]), -10);
-        }
-        if (h_small[0] > S_cap) {                       // more distinct states than the slot layout holds: widen it, run again
+        if (rc) return rc;
+        if (h.n_states > S_cap) {                       // more distinct states than the slot layout holds: widen it, run again
             uint32_t c = S_cap;
-            while (c < h_small[0]) c *= 2;
+            while (c < h.n_states) c *= 2;
             ctx->state_cap = std::min<uint32_t>(c, MAX_STATES);
             if (attempt > 4) return fail(ctx, "state capacity did not converge");
             continue;
         }
-        if (h_small[3] > R.rows_cap) {                  // more rows than the buffer holds: grow it, emit again
-            CK(ctx->d_rows.ensure((size_t)h_small[3] * sizeof(mkp_row)));
-            R.rows = ctx->d_rows.as<mkp_row>(); R.rows_cap = (uint32_t)std::min<size_t>(0xffffffffu, ctx->d_rows.cap / sizeof(mkp_row));
-            ctx->launches += 1;
-            k_rows<true><<<rg, 256, 0, st>>>(R);
-            CK(cudaEventRecord(ctx->ev[3], st));
+        if (h.n_rows > R.rows_cap) {                    // more rows than the buffer holds: grow it, emit again
+            CK(ctx->d_rows.ensure((size_t)h.n_rows * sizeof(mkp_row)));
+            R = row_dev(ctx, C, stride, S_cap);
+            launch(ctx, k_rows<true>, rg, 256, 0, st, R);
+            CK(cudaEventRecord(ctx->ev[9], st));
             CK(cudaStreamSynchronize(st));
             CK(cudaGetLastError());
         }
         break;
     }
-    ctx->n_rows = h_small[3];
+    ctx->n_rows = h.n_rows;
     ctx->pass_prof[3] += 1;
     if (stats) {
         memset(stats, 0, sizeof *stats);
-        stats->n_rows = h_small[3]; stats->n_hot = n_hot; stats->n_calls = h_calls; stats->n_states = h_small[0];
-        stats->n_reads_skipped = h_slow;            // reads that went through the generic kernels
-        auto el = [&](int a, int b) { float ms = 0; cudaEventElapsedTime(&ms, ctx->ev[a], ctx->ev[b]); return ms; };
-        // kernel_ms: 0 parse (fused: the fused pass), incl. the clearing of the slots; 1 resolve (fused: generic kernels over the listed
-        // reads); 4 counters; 5 rows; 6 host syncs (none on this path); 7 total
-        stats->kernel_ms[0] = el(0, 1); stats->kernel_ms[1] = el(1, 2); stats->kernel_ms[4] = el(2, 4); stats->kernel_ms[5] = el(4, 3); stats->kernel_ms[7] = el(0, 3);
-        if (!fused_ran) stats->n_reads_skipped = 0;
+        stats->n_rows = h.n_rows; stats->n_hot = n_hot; stats->n_calls = h.total_calls; stats->n_states = h.n_states;
+        stats->n_reads_skipped = use_fused ? h.work[4] : 0;      // reads the fused kernel left to the generic kernels
+        pass_ms(ctx, false, stats->kernel_ms);
     }
     return 0;
 }
 
+// The hot-mark pass, for chunks without focus bitmaps: k_resolve marks the (position, strand) of every call, and the rank of the
+// marks gives the counter slots. The host reads back the slot and state counts before it sizes the slots, and the row count
+// before it sizes the rows.
 int mkp_pileup_resident(mkp_ctx* ctx, mkp_stats* stats) {
     if (!ctx) return -1;
     if (!ctx->have_params) return fail(ctx, "mkp_set_params was not called");
     if (ctx->ce <= ctx->cs) return fail(ctx, "no resident chunk");
     CK(cudaSetDevice(ctx->device));
-    if (ctx->have_focus && ctx->focus_ready && !getenv("MKP_NO_FOCUS_RANK")) return pileup_fused(ctx, stats);
+    if (ctx->have_focus && ctx->focus_ready && !getenv("MKP_NO_FOCUS_RANK")) return pileup_focus(ctx, stats);
     cudaStream_t st = ctx->stream;
     ChunkDev C;
     const int grid = decode_grid(ctx, ctx->n_reads);
-    if (int rc = prepare_decode(ctx, &C, grid)) return rc;
+    if (int rc = prepare_decode(ctx, &C, grid, MODE_PILEUP)) return rc;
     const uint32_t n_words = ctx->n_words;
-    const uint32_t n_blk = (n_words + 1023) / 1024;
-    CK(ctx->d_block_sums.ensure((size_t)n_blk * 4 + 4));
     CK(ctx->d_row_counts.ensure((size_t)n_words * 4 + 4));
     CK(ctx->d_row_prefix.ensure((size_t)n_words * 4 + 4));
-
-    // events: 0 start | 1 after parse | 2 after resolve | 3 after rank | 4 before counts | 5 after count_calls |
-    //         6 after count_bases | 7 after row count+scan | 8 before emit | 9 end
+    PassScratch* const s = ctx->d_small.as<PassScratch>();
     CK(cudaEventRecord(ctx->ev[0], st));
-    CK(cudaMemsetAsync(ctx->d_hot.p, 0, (size_t)n_words * 8, st));
-    CK(cudaMemsetAsync(ctx->d_small.p, 0xff, 32 * 8, st));
-    CK(cudaMemsetAsync(ctx->d_small.as<uint8_t>() + 32 * 8, 0, SMALL_BYTES - 32 * 8, st));
-    C.mode = MODE_PILEUP;
-    ctx->launches += 1; if (ctx->n_reads) k_parse<<<grid, 128, 0, st>>>(C);
-    CK(cudaEventRecord(ctx->ev[1], st));
-    ctx->launches += 2; if (ctx->n_reads) { k_resolve<MODE_PILEUP, true><<<grid, 128, 0, st>>>(C); k_resolve<MODE_PILEUP, false><<<grid, 128, 0, st>>>(C); }
-    CK(cudaEventRecord(ctx->ev[2], st));
+    CK(cudaMemsetAsync(C.hot, 0, (size_t)n_words * 8, st));
+    if (int rc = clear_scratch(ctx)) return rc;
+    if (int rc = decode(ctx, C, grid)) return rc;
     // counter slot of every marked (position, strand): its rank in the [2][n_words] per-strand marks
-    uint32_t* u = (uint32_t*)(ctx->d_small.as<uint8_t>() + 34 * 8);   // n_states, err, n_hot, n_rows
-    const uint32_t n_blk2 = (2 * n_words + 1023) / 1024;
-    CK(ctx->d_block_sums.ensure((size_t)n_blk2 * 4 + 4));
-    ctx->launches += 1; k_block_popc<<<n_blk2, 1024, 0, st>>>(C.hot, 2 * n_words, ctx->d_block_sums.as<uint32_t>(), C.focus_pos, C.focus_neg);
-    ctx->launches += 1; k_scan_blocks<<<1, 1024, 0, st>>>(ctx->d_block_sums.as<uint32_t>(), n_blk2, u + 2);
-    ctx->launches += 1; k_word_prefix<<<n_blk2, 1024, 0, st>>>(C.hot, 2 * n_words, ctx->d_block_sums.as<uint32_t>(), C.hot_prefix);
-    ctx->launches += 1; k_word_record<<<(n_words + 255) / 256, 256, 0, st>>>(C.hot, C.hot_prefix, n_words, ctx->d_wrec.as<uint4>());
+    if (int rc = rank_bits(ctx, C.hot, 2 * n_words, C.focus_pos, C.focus_neg, C.hot_prefix, &s->n_hot)) return rc;
+    launch(ctx, k_word_record, (n_words + 255) / 256, 256, 0, st, C.hot, C.hot_prefix, n_words, ctx->d_wrec.as<uint4>());
     CK(cudaEventRecord(ctx->ev[3], st));
-    uint32_t h_small[4];
-    unsigned long long h_calls = 0;
-    CK(cudaMemcpyAsync(h_small, u, 16, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&h_calls, C.total_calls, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    const uint32_t n_states = h_small[0], derr = h_small[1], n_hot = h_small[2];
-    if (derr) {
-        if (stats) { memset(stats, 0, sizeof *stats); stats->device_error = derr; }
-        return fail(ctx, "device decode error: " + derr_text(derr), -10);
-    }
-    const uint32_t stride = SL_MOD + std::max<uint32_t>(n_states, 1);
+    PassScratch h;
+    if (int rc = finish_status(ctx, stats, &h)) return rc;
+    const uint32_t n_hot = h.n_hot, n_states = std::max<uint32_t>(h.n_states, 1);
+    const uint32_t stride = SL_MOD + n_states;
     CK(ctx->d_slots.ensure(std::max<size_t>(1, n_hot) * stride * 4));
     CK(cudaMemsetAsync(ctx->d_slots.p, 0, (size_t)n_hot * stride * 4, st));
     CK(ctx->d_obs_word.ensure((size_t)n_words * 8 + 8));
     CK(cudaMemsetAsync(ctx->d_obs_word.p, 0, (size_t)n_words * 8, st));
-    CountDev D;
-    D.hdrs = C.hdrs; D.heap = C.heap; D.meta = C.meta; D.calls = C.calls; D.n_reads = C.n_reads; D.cs = C.cs; D.ce = C.ce;
-    D.rec = ctx->d_wrec.as<uint4>();
-    D.slots = ctx->d_slots.as<uint32_t>(); D.stride = stride; D.n_states = std::max<uint32_t>(n_states, 1);
-    D.n_words = n_words; D.obs_word = ctx->d_obs_word.as<uint32_t>(); D.work = u + 6;
-    D.list = nullptr; D.list_count = nullptr; D.order = nullptr;      // (the counting kernels keep the coordinate order: neighbouring reads update neighbouring slots)
     CK(cudaEventRecord(ctx->ev[4], st));
-    const int g2 = std::max(1, std::min(ctx->sm_count * 8, (int)((ctx->n_reads + 7) / 8)));
-    // the two counting kernels only meet in commutative atomics on the slots: run them side by side (both are
-    // latency-bound at 32 registers, so they co-reside on the SMs)
-    CK(cudaEventRecord(ctx->ev_fork, st));
-    CK(cudaStreamWaitEvent(ctx->stream2, ctx->ev_fork, 0));
-    ctx->launches += 1; if (ctx->n_reads && n_hot) k_count_calls<<<g2, 256, 0, ctx->stream2>>>(D);
-    CK(cudaEventRecord(ctx->ev_join, ctx->stream2));
-    CK(cudaEventRecord(ctx->ev[5], st));
-    ctx->launches += 1; if (ctx->n_reads && n_hot) k_count_bases<<<g2, 256, 0, st>>>(D);
-    CK(cudaStreamWaitEvent(st, ctx->ev_join, 0));
+    if (ctx->n_reads && n_hot) {
+        if (int rc = count_side_by_side(ctx, count_dev(ctx, C, stride, n_states))) return rc;
+    }
     CK(cudaEventRecord(ctx->ev[6], st));
-    RowDev R;
-    R.rec = D.rec; R.n_words = n_words; R.cs = C.cs; R.ce = C.ce;
-    R.slots = D.slots; R.stride = stride; R.n_states = D.n_states; R.states = C.states; R.numeric_mode = ctx->params.numeric_mode;
-    R.obs_word = D.obs_word;
-    R.row_counts = ctx->d_row_counts.as<uint32_t>(); R.row_prefix = ctx->d_row_prefix.as<uint32_t>(); R.rows = nullptr;
+    RowDev R = row_dev(ctx, C, stride, n_states);
     const int rg = (n_words + 255) / 256;
-    ctx->launches += 1; k_rows<false><<<rg, 256, 0, st>>>(R);
-    ctx->launches += 1; k_block_sum<<<n_blk, 1024, 0, st>>>(R.row_counts, n_words, ctx->d_block_sums.as<uint32_t>());
-    ctx->launches += 1; k_scan_blocks<<<1, 1024, 0, st>>>(ctx->d_block_sums.as<uint32_t>(), n_blk, u + 3);
-    ctx->launches += 1; k_value_prefix<<<n_blk, 1024, 0, st>>>(R.row_counts, n_words, ctx->d_block_sums.as<uint32_t>(), ctx->d_row_prefix.as<uint32_t>());
+    launch(ctx, k_rows<false>, rg, 256, 0, st, R);
+    if (int rc = exclusive_scan_u32(ctx, R.row_counts, n_words, ctx->d_row_prefix.as<uint32_t>(), &s->n_rows)) return rc;
     CK(cudaEventRecord(ctx->ev[7], st));
-    uint32_t n_rows = 0;
-    CK(cudaMemcpyAsync(&n_rows, u + 3, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    CK(ctx->d_rows.ensure(std::max<size_t>(1, n_rows) * sizeof(mkp_row)));
-    R.rows = ctx->d_rows.as<mkp_row>(); R.rows_cap = 0xffffffffu;
+    if (int rc = read_scratch(ctx, &h)) return rc;
+    CK(ctx->d_rows.ensure(std::max<size_t>(1, h.n_rows) * sizeof(mkp_row)));
+    R = row_dev(ctx, C, stride, n_states);
     CK(cudaEventRecord(ctx->ev[8], st));
-    ctx->launches += 1; if (n_rows) k_rows<true><<<rg, 256, 0, st>>>(R);
+    if (h.n_rows) launch(ctx, k_rows<true>, rg, 256, 0, st, R);
     CK(cudaEventRecord(ctx->ev[9], st));
     CK(cudaStreamSynchronize(st));
     CK(cudaGetLastError());
-    ctx->n_rows = n_rows;
+    ctx->n_rows = h.n_rows;
     if (stats) {
         memset(stats, 0, sizeof *stats);
-        stats->n_rows = n_rows; stats->n_hot = n_hot; stats->n_calls = h_calls; stats->n_states = n_states;
-        // kernel_ms: 0 parse, 1 resolve, 2 rank, 3 count_calls, 4 count_bases, 5 rows (count+scan+emit), 6 host syncs/allocs, 7 total
-        auto el = [&](int a, int b) { float ms = 0; cudaEventElapsedTime(&ms, ctx->ev[a], ctx->ev[b]); return ms; };
-        stats->kernel_ms[0] = el(0, 1); stats->kernel_ms[1] = el(1, 2); stats->kernel_ms[2] = el(2, 3);
-        stats->kernel_ms[3] = 0.f; stats->kernel_ms[4] = el(4, 6);   // count_calls overlaps count_bases: [4] is the pair
-        stats->kernel_ms[5] = el(6, 7) + el(8, 9);
-        stats->kernel_ms[6] = el(3, 4) + el(7, 8); stats->kernel_ms[7] = el(0, 9);
+        stats->n_rows = h.n_rows; stats->n_hot = n_hot; stats->n_calls = h.total_calls; stats->n_states = h.n_states;
+        pass_ms(ctx, true, stats->kernel_ms);
     }
     return 0;
 }
@@ -644,10 +678,8 @@ int mkp_hemi_resident(mkp_ctx* ctx, const uint32_t* interval_starts, uint32_t n_
     cudaStream_t st = ctx->stream;
     ChunkDev C;
     const int grid = decode_grid(ctx, ctx->n_reads);
-    if (int rc = prepare_decode(ctx, &C, grid)) return rc;
+    if (int rc = prepare_decode(ctx, &C, grid, MODE_PILEUP)) return rc;
     const uint32_t n_words = ctx->n_words;
-    const uint32_t n_blk = (n_words + 1023) / 1024;
-    CK(ctx->d_block_sums.ensure((size_t)n_blk * 4 + 4));
     CK(ctx->d_row_counts.ensure((size_t)n_words * 4 + 4));
     CK(ctx->d_row_prefix.ensure((size_t)n_words * 4 + 4));
     CK(ctx->d_iv_start.ensure((size_t)n_intervals * 4));
@@ -656,36 +688,18 @@ int mkp_hemi_resident(mkp_ctx* ctx, const uint32_t* interval_starts, uint32_t n_
     C.hot = ctx->d_hemi_hot.as<uint32_t>();
     uint32_t* const focus = ctx->d_focus_pos.as<uint32_t>();
     uint32_t* const focus_prefix = ctx->d_hemi_prefix.as<uint32_t>();
-
-    // events: 0 start | 1 after parse | 2 after resolve | 3 after rank | 4 before counts | 6 after counts | 7 after row count+scan
-    //         | 8 before emit | 9 end
+    PassScratch* const s = ctx->d_small.as<PassScratch>();
     CK(cudaEventRecord(ctx->ev[0], st));
     CK(cudaMemcpyAsync(ctx->d_iv_start.p, interval_starts, (size_t)n_intervals * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemsetAsync(C.hot, 0, (size_t)n_words * 8, st));
-    CK(cudaMemsetAsync(ctx->d_small.p, 0xff, 32 * 8, st));
-    CK(cudaMemsetAsync(ctx->d_small.as<uint8_t>() + 32 * 8, 0, SMALL_BYTES - 32 * 8, st));
-    C.mode = MODE_PILEUP;
-    ctx->launches += 1; if (ctx->n_reads) k_parse<<<grid, 128, 0, st>>>(C);
-    CK(cudaEventRecord(ctx->ev[1], st));
-    ctx->launches += 2; if (ctx->n_reads) { k_resolve<MODE_PILEUP, true><<<grid, 128, 0, st>>>(C); k_resolve<MODE_PILEUP, false><<<grid, 128, 0, st>>>(C); }
-    CK(cudaEventRecord(ctx->ev[2], st));
+    if (int rc = clear_scratch(ctx)) return rc;
+    if (int rc = decode(ctx, C, grid)) return rc;
     // counter slot of every + strand motif position: its rank in focus_pos (k_block_popc without focus bitmaps only reads it)
-    uint32_t* u = (uint32_t*)(ctx->d_small.as<uint8_t>() + 34 * 8);   // n_states, err, n_hot, n_rows
-    ctx->launches += 1; k_block_popc<<<n_blk, 1024, 0, st>>>(focus, n_words, ctx->d_block_sums.as<uint32_t>(), nullptr, nullptr);
-    ctx->launches += 1; k_scan_blocks<<<1, 1024, 0, st>>>(ctx->d_block_sums.as<uint32_t>(), n_blk, u + 2);
-    ctx->launches += 1; k_word_prefix<<<n_blk, 1024, 0, st>>>(focus, n_words, ctx->d_block_sums.as<uint32_t>(), focus_prefix);
+    if (int rc = rank_bits(ctx, focus, n_words, nullptr, nullptr, focus_prefix, &s->n_hot)) return rc;
     CK(cudaEventRecord(ctx->ev[3], st));
-    uint32_t h_small[4];
-    unsigned long long h_calls = 0;
-    CK(cudaMemcpyAsync(h_small, u, 16, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&h_calls, C.total_calls, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    const uint32_t n_states = h_small[0], derr = h_small[1], n_hot = h_small[2];
-    if (derr) {
-        if (stats) { memset(stats, 0, sizeof *stats); stats->device_error = derr; }
-        return fail(ctx, "device decode error: " + derr_text(derr), -10);
-    }
-    const uint32_t n_sides = n_states + 1;
+    PassScratch h;
+    if (int rc = finish_status(ctx, stats, &h)) return rc;
+    const uint32_t n_hot = h.n_hot, n_sides = h.n_states + 1;
     const uint32_t stride = 1 + 4 * hemi_base_words(n_sides);
     CK(ctx->d_slots.ensure(std::max<size_t>(1, n_hot) * stride * 4));
     CK(cudaMemsetAsync(ctx->d_slots.p, 0, (size_t)n_hot * stride * 4, st));
@@ -696,39 +710,31 @@ int mkp_hemi_resident(mkp_ctx* ctx, const uint32_t* interval_starts, uint32_t n_
     D.partner = partner_offset;
     D.slots = ctx->d_slots.as<uint32_t>(); D.stride = stride; D.n_sides = n_sides;
     D.scr_cq = C.scr_cq; D.scr_cr = C.scr_cr; D.scr_stride = ctx->max_ncigar + 4;     // prepare_decode sized them for `grid` blocks of 4 warps
-    D.work = u + 6;
+    D.work = C.work + 2;
     CK(cudaEventRecord(ctx->ev[4], st));
-    ctx->launches += 1; if (ctx->n_reads && n_hot) k_hemi_count<<<grid, 128, 0, st>>>(D);
+    if (ctx->n_reads && n_hot) launch(ctx, k_hemi_count, grid, 128, 0, st, D);
     CK(cudaEventRecord(ctx->ev[6], st));
     HemiRowDev R;
     R.focus = focus; R.focus_prefix = focus_prefix; R.n_words = n_words; R.cs = C.cs;
     R.slots = D.slots; R.stride = stride; R.n_sides = n_sides; R.states = C.states; R.combine = ctx->params.numeric_mode == 1;
     R.row_counts = ctx->d_row_counts.as<uint32_t>(); R.row_prefix = ctx->d_row_prefix.as<uint32_t>(); R.rows = nullptr;
     const int rg = (n_words + 255) / 256;
-    ctx->launches += 1; k_hemi_rows<false><<<rg, 256, 0, st>>>(R);
-    ctx->launches += 1; k_block_sum<<<n_blk, 1024, 0, st>>>(R.row_counts, n_words, ctx->d_block_sums.as<uint32_t>());
-    ctx->launches += 1; k_scan_blocks<<<1, 1024, 0, st>>>(ctx->d_block_sums.as<uint32_t>(), n_blk, u + 3);
-    ctx->launches += 1; k_value_prefix<<<n_blk, 1024, 0, st>>>(R.row_counts, n_words, ctx->d_block_sums.as<uint32_t>(), ctx->d_row_prefix.as<uint32_t>());
+    launch(ctx, k_hemi_rows<false>, rg, 256, 0, st, R);
+    if (int rc = exclusive_scan_u32(ctx, R.row_counts, n_words, ctx->d_row_prefix.as<uint32_t>(), &s->n_rows)) return rc;
     CK(cudaEventRecord(ctx->ev[7], st));
-    uint32_t n_rows = 0;
-    CK(cudaMemcpyAsync(&n_rows, u + 3, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    CK(ctx->d_hemi_rows.ensure(std::max<size_t>(1, n_rows) * sizeof(mkp_hemi_row)));
+    if (int rc = read_scratch(ctx, &h)) return rc;
+    CK(ctx->d_hemi_rows.ensure(std::max<size_t>(1, h.n_rows) * sizeof(mkp_hemi_row)));
     R.rows = ctx->d_hemi_rows.as<mkp_hemi_row>();
     CK(cudaEventRecord(ctx->ev[8], st));
-    ctx->launches += 1; if (n_rows) k_hemi_rows<true><<<rg, 256, 0, st>>>(R);
+    if (h.n_rows) launch(ctx, k_hemi_rows<true>, rg, 256, 0, st, R);
     CK(cudaEventRecord(ctx->ev[9], st));
     CK(cudaStreamSynchronize(st));
     CK(cudaGetLastError());
-    ctx->n_hemi_rows = n_rows;
+    ctx->n_hemi_rows = h.n_rows;
     if (stats) {
         memset(stats, 0, sizeof *stats);
-        stats->n_rows = n_rows; stats->n_hot = n_hot; stats->n_calls = h_calls; stats->n_states = n_states;
-        // kernel_ms: 0 parse, 1 resolve, 2 rank, 4 counters (k_hemi_count), 5 rows (count+scan+emit), 6 host syncs/allocs, 7 total
-        auto el = [&](int a, int b) { float ms = 0; cudaEventElapsedTime(&ms, ctx->ev[a], ctx->ev[b]); return ms; };
-        stats->kernel_ms[0] = el(0, 1); stats->kernel_ms[1] = el(1, 2); stats->kernel_ms[2] = el(2, 3);
-        stats->kernel_ms[4] = el(4, 6); stats->kernel_ms[5] = el(6, 7) + el(8, 9);
-        stats->kernel_ms[6] = el(3, 4) + el(7, 8); stats->kernel_ms[7] = el(0, 9);
+        stats->n_rows = h.n_rows; stats->n_hot = n_hot; stats->n_calls = h.total_calls; stats->n_states = h.n_states;
+        pass_ms(ctx, true, stats->kernel_ms);
     }
     return 0;
 }
@@ -749,90 +755,65 @@ int mkp_pileup_chunk(mkp_ctx* ctx, const mkp_chunk* ch, const mkp_row** rows, si
     return mkp_fetch_rows(ctx, rows, n_rows);
 }
 
-int mkp_sample_histogram(mkp_ctx* ctx, int include_unaligned, const uint8_t* take, uint64_t* hist, uint8_t* contributes, uint64_t* inexact) {
-    if (!ctx) return -1;
+// The sampling decode (MODE_HIST) of the resident chunk, over the reads flagged in `take` (every read if null). `out_words` u64
+// counters at d_hist are zeroed and attached as C.summ (`summary`) or C.hist; none if 0. The caller enqueues its copies back,
+// then finish_status.
+static int sample_decode(mkp_ctx* ctx, int include_unaligned, const uint8_t* take, bool summary, size_t out_words) {
     if (!ctx->have_params) return fail(ctx, "mkp_set_params was not called");
     if (ctx->ce <= ctx->cs) return fail(ctx, "no resident chunk");
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     ChunkDev C;
     const int grid = decode_grid(ctx, ctx->n_reads);
-    if (int rc = prepare_decode(ctx, &C, grid)) return rc;
-    CK(cudaMemsetAsync(ctx->d_small.p, 0xff, 32 * 8, st));
-    CK(cudaMemsetAsync(ctx->d_small.as<uint8_t>() + 32 * 8, 0, SMALL_BYTES - 32 * 8, st));
+    if (int rc = prepare_decode(ctx, &C, grid, MODE_HIST)) return rc;
+    if (int rc = clear_scratch(ctx)) return rc;
     C.hist_include_unaligned = include_unaligned ? 1 : 0;
     if (take) {
         CK(ctx->d_take.ensure(std::max<size_t>(1, ctx->n_reads)));
         CK(cudaMemcpyAsync(ctx->d_take.p, take, ctx->n_reads, cudaMemcpyHostToDevice, st));
         C.take = ctx->d_take.as<uint8_t>();
     }
-    if (hist) {
-        CK(ctx->d_hist.ensure(4 * 1025 * 8));
-        CK(cudaMemsetAsync(ctx->d_hist.p, 0, 4 * 1025 * 8, st));
-        C.hist = ctx->d_hist.as<unsigned long long>();
+    if (out_words) {
+        CK(ctx->d_hist.ensure(std::max<size_t>(4 * 1025, out_words) * 8));     // one size for both uses: no regrowth between them
+        CK(cudaMemsetAsync(ctx->d_hist.p, 0, out_words * 8, st));
+        if (summary) C.summ = ctx->d_hist.as<unsigned long long>();
+        else C.hist = ctx->d_hist.as<unsigned long long>();
     }
-    C.mode = MODE_HIST;
-    ctx->launches += 3; if (ctx->n_reads) { k_parse<<<grid, 128, 0, st>>>(C); k_resolve<MODE_HIST, true><<<grid, 128, 0, st>>>(C); k_resolve<MODE_HIST, false><<<grid, 128, 0, st>>>(C); }
-    CK(cudaGetLastError());
-    uint32_t h_small[2];
-    uint32_t* u = (uint32_t*)(ctx->d_small.as<uint8_t>() + 34 * 8);
-    CK(cudaMemcpyAsync(h_small, u, 8, cudaMemcpyDeviceToHost, st));
-    if (hist) CK(cudaMemcpyAsync(hist, ctx->d_hist.p, 4 * 1025 * 8, cudaMemcpyDeviceToHost, st));
-    unsigned long long inx = 0;
-    CK(cudaMemcpyAsync(&inx, C.hist_inexact, 8, cudaMemcpyDeviceToHost, st));
+    return decode(ctx, C, grid);
+}
+
+int mkp_sample_histogram(mkp_ctx* ctx, int include_unaligned, const uint8_t* take, uint64_t* hist, uint8_t* contributes, uint64_t* inexact) {
+    if (!ctx) return -1;
+    if (int rc = sample_decode(ctx, include_unaligned, take, false, hist ? 4 * 1025 : 0)) return rc;
+    if (hist) CK(cudaMemcpyAsync(hist, ctx->d_hist.p, 4 * 1025 * 8, cudaMemcpyDeviceToHost, ctx->stream));
     std::vector<ReadMeta> metas;
     if (contributes) {
         metas.resize(ctx->n_reads);
-        if (ctx->n_reads) CK(cudaMemcpyAsync(metas.data(), ctx->d_meta.p, (size_t)ctx->n_reads * sizeof(ReadMeta), cudaMemcpyDeviceToHost, st));
+        if (ctx->n_reads) CK(cudaMemcpyAsync(metas.data(), ctx->d_meta.p, (size_t)ctx->n_reads * sizeof(ReadMeta), cudaMemcpyDeviceToHost, ctx->stream));
     }
-    CK(cudaStreamSynchronize(st));
-    if (h_small[1]) return fail(ctx, "device decode error: " + derr_text(h_small[1]), -10);
+    PassScratch h;
+    if (int rc = finish_status(ctx, nullptr, &h)) return rc;
     if (contributes) for (uint32_t i = 0; i < ctx->n_reads; i++) contributes[i] = metas[i].n_hist > 0;
-    if (inexact) *inexact = inx;
+    if (inexact) *inexact = h.hist_inexact;
     return 0;
 }
-
 
 // `modkit summary` support: the calls of the reads flagged in `take`, classed with the thresholds of mkp_set_params
 // (src/summarize.rs:117-252). Adds to table[4][2][33] (base, pass/fail, 0 canonical | 1 + state), reads_with[4], obs[4];
 // states[32] receives the (base << 32 | code) key of every state id (~0 = unused).
 int mkp_sample_summary(mkp_ctx* ctx, int include_unaligned, const uint8_t* take, uint64_t* table, uint64_t* reads_with, uint32_t* obs, uint64_t* states) {
     if (!ctx || !table || !reads_with || !obs || !states) return -1;
-    if (!ctx->have_params) return fail(ctx, "mkp_set_params was not called");
-    if (ctx->ce <= ctx->cs) return fail(ctx, "no resident chunk");
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->stream;
-    ChunkDev C;
-    const int grid = decode_grid(ctx, ctx->n_reads);
-    if (int rc = prepare_decode(ctx, &C, grid)) return rc;
-    CK(cudaMemsetAsync(ctx->d_small.p, 0xff, 32 * 8, st));
-    CK(cudaMemsetAsync(ctx->d_small.as<uint8_t>() + 32 * 8, 0, SMALL_BYTES - 32 * 8, st));
-    C.hist_include_unaligned = include_unaligned ? 1 : 0;
-    if (take) {
-        CK(ctx->d_take.ensure(std::max<size_t>(1, ctx->n_reads)));
-        CK(cudaMemcpyAsync(ctx->d_take.p, take, ctx->n_reads, cudaMemcpyHostToDevice, st));
-        C.take = ctx->d_take.as<uint8_t>();
-    }
     const size_t words = 4 * 2 * 33 + 4 + 2;
-    CK(ctx->d_hist.ensure(std::max<size_t>(4 * 1025, words) * 8));
-    CK(cudaMemsetAsync(ctx->d_hist.p, 0, words * 8, st));
-    C.summ = ctx->d_hist.as<unsigned long long>();
-    C.mode = MODE_HIST;
-    ctx->launches += 3;
-    if (ctx->n_reads) { k_parse<<<grid, 128, 0, st>>>(C); k_resolve<MODE_HIST, true><<<grid, 128, 0, st>>>(C); k_resolve<MODE_HIST, false><<<grid, 128, 0, st>>>(C); }
-    CK(cudaGetLastError());
-    std::vector<uint64_t> h(words);
-    uint32_t h_small[2];
-    uint32_t* u = (uint32_t*)(ctx->d_small.as<uint8_t>() + 34 * 8);
-    CK(cudaMemcpyAsync(h_small, u, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(h.data(), ctx->d_hist.p, words * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(states, ctx->d_small.p, 32 * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (h_small[1]) return fail(ctx, "device decode error: " + derr_text(h_small[1]), -10);
-    for (int i = 0; i < 4 * 2 * 33; i++) table[i] += h[i];
-    for (int b = 0; b < 4; b++) reads_with[b] += h[4 * 2 * 33 + b];
-    const uint32_t* o32 = (const uint32_t*)(h.data() + 4 * 2 * 33 + 4);
+    if (int rc = sample_decode(ctx, include_unaligned, take, true, words)) return rc;
+    std::vector<uint64_t> hv(words);
+    CK(cudaMemcpyAsync(hv.data(), ctx->d_hist.p, words * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    PassScratch h;
+    if (int rc = finish_status(ctx, nullptr, &h)) return rc;
+    for (int i = 0; i < 4 * 2 * 33; i++) table[i] += hv[i];
+    for (int b = 0; b < 4; b++) reads_with[b] += hv[4 * 2 * 33 + b];
+    const uint32_t* o32 = (const uint32_t*)(hv.data() + 4 * 2 * 33 + 4);
     for (int b = 0; b < 4; b++) obs[b] = o32[b];
+    memcpy(states, h.states, sizeof h.states);
     return 0;
 }
 
@@ -936,14 +917,12 @@ static int bam_load_range_impl(mkp_ctx* ctx, HostSrc hs, size_t file_len, const 
     CK(ctx->d_seeds.ensure(n_seeds * 8));
     CK(ctx->d_seg_counts.ensure(n_seeds * 4 + 4));
     CK(ctx->d_seg_base.ensure(n_seeds * 4 + 4));
-    CK(ctx->d_small.ensure(SMALL_BYTES));
-    const uint32_t n_blk = (uint32_t)((n_seeds + 1023) / 1024);
-    CK(ctx->d_block_sums.ensure((size_t)n_blk * 4 + 4));
-    uint32_t* u = (uint32_t*)(ctx->d_small.as<uint8_t>() + 34 * 8);    // u+10 status, u+11 work, u+12 record count
+    CK(ctx->d_small.ensure(sizeof(PassScratch)));
+    PassScratch* const s = ctx->d_small.as<PassScratch>();
     CK(cudaEventRecord(ctx->ev[0], st));
     CK(cudaMemcpyAsync(ctx->d_members.p, members, n_members * sizeof(mkp_bgzf_member), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->d_seeds.p, seeds, n_seeds * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(u + 10, 0, 12, st));
+    CK(cudaMemsetAsync(&s->ingest_status, 0, sizeof s->ingest_status, st));
     // decoder tables in shared memory (MKP_INFLATE_SMEM=1) or in an L2-resident global scratch (default): see k_inflate
     static const bool tab_global = !(getenv("MKP_INFLATE_SMEM") && getenv("MKP_INFLATE_SMEM")[0] == '1');
     int warps_sm = 28;
@@ -993,35 +972,28 @@ static int bam_load_range_impl(mkp_ctx* ctx, HostSrc hs, size_t file_len, const 
         CK(cudaStreamWaitEvent(st, ctx->ev_join, 0));
         const size_t nm = cut[sl + 1] - cut[sl];
         const int grid = (int)std::min<size_t>((nm + INF_THREADS - 1) / INF_THREADS, (size_t)ctx->sm_count * per_sm);
-        ctx->launches += 1; k_inflate<<<grid, INF_THREADS, smem, st>>>(ctx->d_file.as<uint8_t>(), ctx->d_members.as<mkp_bgzf_member>() + cut[sl], (uint32_t)nm,
-                                                  ctx->d_bam.as<uint8_t>(), u + 10, ctx->d_slab_work.as<uint32_t>() + sl, (uint32_t)cut[sl], gtab, hdr_batch);
+        launch(ctx, k_inflate, grid, INF_THREADS, smem, st, ctx->d_file.as<uint8_t>(), ctx->d_members.as<mkp_bgzf_member>() + cut[sl], (uint32_t)nm,
+               ctx->d_bam.as<uint8_t>(), &s->ingest_status, ctx->d_slab_work.as<uint32_t>() + sl, (uint32_t)cut[sl], gtab, hdr_batch);
     }
     CK(cudaEventRecord(ctx->ev[1], ctx->stream2));
     CK(cudaEventRecord(ctx->ev[2], st));
     const int wg = (int)((n_seeds + 127) / 128);
-    ctx->launches += 1; k_walk<0><<<wg, 128, 0, st>>>(ctx->d_bam.as<uint8_t>(), walk_end, ctx->d_seeds.as<uint64_t>(), (uint32_t)n_seeds,
-                                  ctx->d_seg_counts.as<uint32_t>(), nullptr, nullptr, u + 10);
-    ctx->launches += 1; k_block_sum<<<n_blk, 1024, 0, st>>>(ctx->d_seg_counts.as<uint32_t>(), (uint32_t)n_seeds, ctx->d_block_sums.as<uint32_t>());
-    ctx->launches += 1; k_scan_blocks<<<1, 1024, 0, st>>>(ctx->d_block_sums.as<uint32_t>(), n_blk, u + 12);
-    ctx->launches += 1; k_value_prefix<<<n_blk, 1024, 0, st>>>(ctx->d_seg_counts.as<uint32_t>(), (uint32_t)n_seeds, ctx->d_block_sums.as<uint32_t>(), ctx->d_seg_base.as<uint32_t>());
-    uint32_t h[3] = {0, 0, 0};
-    CK(cudaMemcpyAsync(h, u + 10, 12, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    CK(cudaGetLastError());
-    if (h[0]) {
-        const uint32_t e = h[0];
+    launch(ctx, k_walk<0>, wg, 128, 0, st, ctx->d_bam.as<uint8_t>(), walk_end, ctx->d_seeds.as<uint64_t>(), (uint32_t)n_seeds,
+           ctx->d_seg_counts.as<uint32_t>(), nullptr, nullptr, &s->ingest_status);
+    if (int rc = exclusive_scan_u32(ctx, ctx->d_seg_counts.as<uint32_t>(), (uint32_t)n_seeds, ctx->d_seg_base.as<uint32_t>(), &s->n_records)) return rc;
+    PassScratch h;
+    if (int rc = read_scratch(ctx, &h)) return rc;
+    if (const uint32_t e = h.ingest_status) {
         if ((e >> 24) & 0x7f) return fail(ctx, "inflate failed (code " + std::to_string((e >> 24) & 0x7f) + ") in BGZF member " + std::to_string(e & 0xffffffu));
         return fail(ctx, (e & 3u) == 2u ? "record chain does not meet a seed offset (stale or foreign index?)" : "corrupt BAM record in the inflated stream");
     }
-    const size_t nrec = h[2];
+    const size_t nrec = h.n_records;
     CK(ctx->d_recs.ensure(std::max<size_t>(1, nrec) * sizeof(mkp_bam_rec)));
-    ctx->launches += 1; k_walk<1><<<wg, 128, 0, st>>>(ctx->d_bam.as<uint8_t>(), walk_end, ctx->d_seeds.as<uint64_t>(), (uint32_t)n_seeds,
-                                  ctx->d_seg_counts.as<uint32_t>(), ctx->d_seg_base.as<uint32_t>(), ctx->d_recs.as<mkp_bam_rec>(), u + 10);
+    launch(ctx, k_walk<1>, wg, 128, 0, st, ctx->d_bam.as<uint8_t>(), walk_end, ctx->d_seeds.as<uint64_t>(), (uint32_t)n_seeds,
+           ctx->d_seg_counts.as<uint32_t>(), ctx->d_seg_base.as<uint32_t>(), ctx->d_recs.as<mkp_bam_rec>(), &s->ingest_status);
     CK(cudaEventRecord(ctx->ev[3], st));
-    CK(cudaMemcpyAsync(h, u + 10, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    CK(cudaGetLastError());
-    if (h[0]) return fail(ctx, "corrupt BAM record in the inflated stream");
+    if (int rc = read_scratch(ctx, &h)) return rc;
+    if (h.ingest_status) return fail(ctx, "corrupt BAM record in the inflated stream");
     ctx->bam_len = inflated_len;
     ctx->n_records = nrec;
     if (n_records) *n_records = nrec;
@@ -1072,9 +1044,9 @@ int mkp_bam_chunk(mkp_ctx* ctx, uint32_t start, uint32_t end, const uint32_t* re
     if (n) {
         for (uint32_t i = 0; i < n; i++) if (rec_ids[i] >= ctx->n_records) return fail(ctx, "record id out of range");
         CK(cudaMemcpyAsync(ctx->d_ids.p, rec_ids, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-        ctx->launches += 1; k_slice_plan<<<(n + 7) / 8, 256, 0, st>>>(ctx->d_bam.as<uint8_t>(), ctx->d_recs.as<mkp_bam_rec>(), ctx->d_ids.as<uint32_t>(), n,
-                                                     ctx->d_hdrs.as<mkp_read_hdr>(), ctx->d_plan.as<SlicePlan>(), ctx->d_need.as<uint32_t>());
-        ctx->launches += 1; k_slice_scan<<<1, 1024, 0, st>>>(ctx->d_hdrs.as<mkp_read_hdr>(), ctx->d_need.as<uint32_t>(), n, ctx->d_entry_off.as<uint64_t>(), ctx->d_totals.as<uint64_t>());
+        launch(ctx, k_slice_plan, (n + 7) / 8, 256, 0, st, ctx->d_bam.as<uint8_t>(), ctx->d_recs.as<mkp_bam_rec>(), ctx->d_ids.as<uint32_t>(), n,
+               ctx->d_hdrs.as<mkp_read_hdr>(), ctx->d_plan.as<SlicePlan>(), ctx->d_need.as<uint32_t>());
+        launch(ctx, k_slice_scan, 1, 1024, 0, st, ctx->d_hdrs.as<mkp_read_hdr>(), ctx->d_need.as<uint32_t>(), n, ctx->d_entry_off.as<uint64_t>(), ctx->d_totals.as<uint64_t>());
         CK(cudaMemcpyAsync(tot, ctx->d_totals.p, 32, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         CK(cudaGetLastError());
@@ -1082,7 +1054,7 @@ int mkp_bam_chunk(mkp_ctx* ctx, uint32_t start, uint32_t end, const uint32_t* re
         CK(ctx->d_heap.ensure(tot[0] + 64));
         ctx->slice_prof[2] += since(t0); t0 = now();
         const int grid = std::max(1, std::min(ctx->sm_count * 8, (int)((n + 7) / 8)));
-        ctx->launches += 1; k_slice_copy<<<grid, 256, 0, st>>>(ctx->d_bam.as<uint8_t>(), ctx->d_hdrs.as<mkp_read_hdr>(), ctx->d_plan.as<SlicePlan>(), n, ctx->d_heap.as<uint8_t>());
+        launch(ctx, k_slice_copy, grid, 256, 0, st, ctx->d_bam.as<uint8_t>(), ctx->d_hdrs.as<mkp_read_hdr>(), ctx->d_plan.as<SlicePlan>(), n, ctx->d_heap.as<uint8_t>());
     } else {
         CK(cudaMemsetAsync(ctx->d_entry_off.p, 0, 8, st));
         CK(ctx->d_heap.ensure(64));
@@ -1115,21 +1087,18 @@ int mkp_bam_tags(mkp_ctx* ctx, const uint32_t* rec_ids, uint32_t n, const char* 
     for (uint32_t i = 0; i < n; i++) if (rec_ids[i] >= ctx->n_records) return fail(ctx, "record id out of range");
     CK(ctx->d_ids.ensure((size_t)n * 4));
     CK(ctx->d_plan.ensure(std::max<size_t>(sizeof(SlicePlan), (size_t)n * n_tags * MKP_TAG_CELL)));       // (scratch shared with the slicer)
-    CK(ctx->d_small.ensure(SMALL_BYTES));
-    uint32_t* u = (uint32_t*)(ctx->d_small.as<uint8_t>() + 34 * 8);
+    CK(ctx->d_small.ensure(sizeof(PassScratch)));
+    PassScratch* const s = ctx->d_small.as<PassScratch>();
     uint32_t pk[4] = {0, 0, 0, 0};
     for (uint32_t t = 0; t < n_tags; t++) pk[t] = (uint32_t)(uint8_t)tags[2 * t] | ((uint32_t)(uint8_t)tags[2 * t + 1] << 8);
     CK(cudaMemcpyAsync(ctx->d_ids.p, rec_ids, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(u + 14, 0, 4, st));
-    ctx->launches += 1;
-    k_tag_values<<<(n + 7) / 8, 256, 0, st>>>(ctx->d_bam.as<uint8_t>(), ctx->d_recs.as<mkp_bam_rec>(), ctx->d_ids.as<uint32_t>(), n,
-                                                 pk[0] | (pk[1] << 16), pk[2] | (pk[3] << 16), n_tags, ctx->d_plan.as<uint8_t>(), u + 14);
-    uint32_t ovf = 0;
+    CK(cudaMemsetAsync(&s->tag_overflow, 0, sizeof s->tag_overflow, st));
+    launch(ctx, k_tag_values, (n + 7) / 8, 256, 0, st, ctx->d_bam.as<uint8_t>(), ctx->d_recs.as<mkp_bam_rec>(), ctx->d_ids.as<uint32_t>(), n,
+           pk[0] | (pk[1] << 16), pk[2] | (pk[3] << 16), n_tags, ctx->d_plan.as<uint8_t>(), &s->tag_overflow);
     CK(cudaMemcpyAsync(out, ctx->d_plan.p, (size_t)n * n_tags * MKP_TAG_CELL, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&ovf, u + 14, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    CK(cudaGetLastError());
-    if (ovf) return fail(ctx, "a partition tag value is longer than 253 bytes: use --host-ingest for this file");
+    PassScratch h;
+    if (int rc = read_scratch(ctx, &h)) return rc;
+    if (h.tag_overflow) return fail(ctx, "a partition tag value is longer than 253 bytes: use --host-ingest for this file");
     return 0;
 }
 

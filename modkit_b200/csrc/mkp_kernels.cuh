@@ -83,7 +83,9 @@ struct ChunkDev {
     unsigned long long* states; // registry: (pb<<32 | code), ~0 empty
     uint32_t* n_states;
     uint32_t* err;
-    uint32_t* work;             // dynamic read counters: +0 parse, +1 resolve, +2/+3 counts, +4 queue length, +5 queue cursor
+    // dynamic read queues: +0 k_parse, +1 fast k_resolve, +2 k_count_bases / k_hemi_count, +3 k_count_calls (CountDev::work
+    // and HemiDev::work point at +2), +4 length of slow_list, +5 generic k_resolve's cursor in slow_list
+    uint32_t* work;
     uint32_t* slow_list;        // reads left to the generic k_resolve instantiation
     unsigned long long* total_calls;
     // per-warp scratch

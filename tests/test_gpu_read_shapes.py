@@ -398,3 +398,37 @@ def test_declared_limits_at_the_limit_match_oracle(native_lib, oracle_exe, tmp_p
     bam, fa = g.write(tmp_path)
     check_pileup(oracle_exe, ["--ref", fa, "--no-filtering", "--motif", "C", "0", "--motif", "A", "0"], bam, tmp_path, KERNELS, 500)
     check_pileup(oracle_exe, ["--no-filtering"], bam, tmp_path, [None], 500)
+
+
+def test_chunk_without_reads_runs_only_rank_and_row_kernels(native_lib):
+    """A chunk without reads through every pass: no rows, and mkp_kernel_launches counts the kernels issued, which are the
+    rank and row kernels only. Decode, counting and emit kernels have nothing to do and are not launched."""
+    import numpy as np
+    import modkit_b200
+    ctx = modkit_b200.Context(0)
+    ctx.set_params(modkit_b200.make_params())
+    end = 100000
+    focus = np.zeros((end + 31) // 32, dtype=np.uint32)
+    focus[::7] = 0x01010101
+    for with_focus in (False, True):
+        ch = modkit_b200.Chunk()
+        ch.start, ch.end = 0, end
+        if with_focus:
+            ch.focus_pos = ch.focus_neg = focus.ctypes.data
+        l0 = ctx.kernel_launches
+        ctx._check(ctx._lib.mkp_upload_chunk(ctx._h, ch))
+        # with focus bitmaps the upload ranks them (3 kernels), builds the word records (1) and the tile table (1)
+        assert ctx.kernel_launches - l0 == (5 if with_focus else 0)
+        l0 = ctx.kernel_launches
+        st = ctx.pileup_resident()
+        assert st.n_rows == 0 and st.n_calls == 0 and len(ctx.fetch_rows()) == 0
+        # hot-mark pass: rank of the marks (3) and word records (1); focus-rank pass: no rank; both: row count and scan (4),
+        # and the focus-rank pass emits without reading the row count back (1)
+        assert ctx.kernel_launches - l0 == (5 if with_focus else 8)
+        l0 = ctx.kernel_launches
+        hist, _, _ = ctx.sample_histogram()
+        assert not hist.any() and ctx.kernel_launches == l0
+    l0 = ctx.kernel_launches
+    st = ctx.hemi_resident([0], 1)
+    assert st.n_rows == 0 and len(ctx.fetch_hemi_rows()) == 0
+    assert ctx.kernel_launches - l0 == 7            # rank of focus_pos (3), row count and scan (4)
