@@ -165,9 +165,18 @@ int  mkp_pileup_chunk(mkp_ctx* ctx, const mkp_chunk* host_chunk, const mkp_row**
  * resident chunk, histogram of the argmax probability of every call of the reads selected by
  * `take` (n_reads flags, host memory; NULL = all), per canonical base, bin = round(p*1024).
  * `contributes[i]` (optional, host memory, n_reads bytes) receives 1 when read i yielded >= 1
- * value.  hist is u64[4][1025]; `inexact` counts values that are not multiples of 1/1024. */
+ * value.  hist is u64[4][1025]; `inexact` counts values that are not multiples of 1/1024 and
+ * values above 1.0 (those are also counted in bin 1024). */
 int  mkp_sample_histogram(mkp_ctx* ctx, int include_unaligned, const uint8_t* take,
                           uint64_t* hist, uint8_t* contributes, uint64_t* inexact);
+
+/* The same with the full range of arg-max values: hist is u64[4][MKP_HIST_BINS], bin k holds
+ * the value k/1024 for k < MKP_HIST_BINS.  Arg-max values above 1.0 are legal: a sum of ML
+ * probabilities up to 1.01, and the share ReDistribute adds to the kept codes, reach ~1.52.
+ * `inexact` counts values off the 1/1024 grid or past the last bin. */
+#define MKP_HIST_BINS 2049
+int  mkp_sample_histogram_wide(mkp_ctx* ctx, int include_unaligned, const uint8_t* take,
+                               uint64_t* hist, uint8_t* contributes, uint64_t* inexact);
 
 
 /* `modkit summary` support (src/summarize.rs:117-252; SURVEY 8f-3): every base-modification call of the reads selected by `take`

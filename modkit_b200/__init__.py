@@ -53,8 +53,10 @@ HEMI_ROW_DTYPE = np.dtype([("pos", "<u4"), ("code_pos", "<u4"), ("code_neg", "<u
                            ("n_diff", "<u4"), ("n_nocall", "<u4")])
 assert HEMI_ROW_DTYPE.itemsize == 44
 
+HIST_BINS = 2049        # MKP_HIST_BINS (include/mkp.h): bins k/1024 of mkp_sample_histogram_wide
+
 MKP_SYMBOLS = ["mkp_create", "mkp_bind_host_thread", "mkp_destroy", "mkp_last_error", "mkp_set_params", "mkp_upload_chunk", "mkp_pileup_resident",
-               "mkp_fetch_rows", "mkp_pileup_chunk", "mkp_sample_histogram", "mkp_sample_summary", "mkp_algorithmic_bytes", "mkp_kernel_launches",
+               "mkp_fetch_rows", "mkp_pileup_chunk", "mkp_sample_histogram", "mkp_sample_histogram_wide", "mkp_sample_summary", "mkp_algorithmic_bytes", "mkp_kernel_launches",
                "mkp_device_memory", "mkp_bam_load", "mkp_bam_load_range", "mkp_bam_load_range_fd", "mkp_bam_records", "mkp_bam_chunk", "mkp_bam_tags", "mkp_bam_inflated", "mkp_fetch_chunk",
                "mkp_hemi_resident", "mkp_fetch_hemi_rows"]
 MKH_SYMBOLS = ["mkh_pileup_main", "mkh_bam_open", "mkh_bam_close", "mkh_bam_n_refs", "mkh_bam_ref_name", "mkh_bam_ref_len",
@@ -98,6 +100,7 @@ def load_library(build_if_missing=True):
     lib.mkh_pileup_hemi_main_sharded.argtypes = [C.c_int, C.POINTER(C.c_char_p), C.c_int, C.c_int, ALLREDUCE_FN, C.c_void_p, C.POINTER(C.c_double)]
     lib.mkp_pileup_chunk.argtypes = [C.c_void_p, C.POINTER(Chunk), C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.POINTER(Stats)]
     lib.mkp_sample_histogram.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
+    lib.mkp_sample_histogram_wide.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
     lib.mkp_sample_summary.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.mkp_algorithmic_bytes.argtypes = [C.POINTER(Chunk), C.c_size_t]
     lib.mkp_algorithmic_bytes.restype = C.c_size_t
@@ -515,8 +518,10 @@ class Context:
         buf = (C.c_uint8 * (40 * n.value)).from_address(rows.value)
         return np.frombuffer(buf, dtype=ROW_DTYPE), st
 
-    def sample_histogram(self, include_unaligned=False, take=None, want_contributes=False):
-        hist = np.zeros((4, 1025), dtype=np.uint64)
+    def sample_histogram(self, include_unaligned=False, take=None, want_contributes=False, wide=False):
+        """(hist, contributes, inexact): hist[base][k] counts the arg-max values k/1024, k <= 1024 (values above 1.0 in bin
+        1024 and in `inexact`), or with wide=True k < HIST_BINS (mkp_sample_histogram_wide)."""
+        hist = np.zeros((4, HIST_BINS if wide else 1025), dtype=np.uint64)
         n = 0
         contrib = None
         inexact = C.c_uint64()
@@ -527,8 +532,9 @@ class Context:
             n = len(take)
         if want_contributes:
             contrib = np.zeros(max(1, self._n_reads_hint), dtype=np.uint8)
-        self._check(self._lib.mkp_sample_histogram(self._h, 1 if include_unaligned else 0, take_p, hist.ctypes.data,
-                                                   contrib.ctypes.data if contrib is not None else None, C.byref(inexact)))
+        fn = self._lib.mkp_sample_histogram_wide if wide else self._lib.mkp_sample_histogram
+        self._check(fn(self._h, 1 if include_unaligned else 0, take_p, hist.ctypes.data,
+                       contrib.ctypes.data if contrib is not None else None, C.byref(inexact)))
         return hist, contrib, inexact.value
 
     _n_reads_hint = 0

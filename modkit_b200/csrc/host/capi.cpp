@@ -44,7 +44,7 @@ int mkh_sample_probs_main(int argc, const char* const* argv) { return sample_mai
 // One rank of an interval-sharded `modkit pileup` (SURVEY 8e): every rank is called with the same arguments (plus its own
 // --device); `allreduce` sums a u64 vector over the ranks in place and returns 0 (NCCL through torch.distributed in
 // bench.py / modkit_b200.pileup_main_sharded; any other transport works). It is called exactly twice per run, in the same
-// order on every rank: the sampled-probability histograms (u64[4*1025 + 2]; thresholds.rs:118-156) and the output slice
+// order on every rank: the sampled-probability histograms (u64[4*MKP_HIST_BINS + 2]; thresholds.rs:118-156) and the output slice
 // sizes (u64[world + 2]); with --include-unmapped a third, one-word exchange precedes them.
 // out_stats (optional, double[20]): total_s, load_s, thresholds_s, gpu_s, write_s, rows (all ranks), positions (all ranks), rows of this
 // rank, base thresholds A C G T (-1 = none), sampler fetch_s, intervals_s, pack_s, kernel_ms, slice_s, pass_s, rowcopy_s.

@@ -741,12 +741,12 @@ inline void focus_bitmaps(const std::vector<RefInterval>& ivs, size_t i0, size_t
     }
 }
 
-// thresholds.rs:17-39 on a histogram whose bins are exact values k/1024
+// thresholds.rs:17-39 on a histogram of MKP_HIST_BINS bins whose bin k holds the exact value k/1024
 inline bool percentile_from_hist(const uint64_t* h, float q, float* out) {
     uint64_t n = 0;
-    for (int k = 0; k <= 1024; k++) n += h[k];
+    for (int k = 0; k < MKP_HIST_BINS; k++) n += h[k];
     if (n < 2) return false;
-    auto value_at = [&](uint64_t idx) { uint64_t acc = 0; for (int k = 0; k <= 1024; k++) { acc += h[k]; if (idx < acc) return (float)k / 1024.0f; } return 1.0f; };
+    auto value_at = [&](uint64_t idx) { uint64_t acc = 0; for (int k = 0; k < MKP_HIST_BINS; k++) { acc += h[k]; if (idx < acc) return (float)k / 1024.0f; } return (float)(MKP_HIST_BINS - 1) / 1024.0f; };
     if (q == 1.0f) { *out = value_at(n - 1); return true; }
     const float l = (float)(n - 1);
     const float x = l * q;

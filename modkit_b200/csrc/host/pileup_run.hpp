@@ -203,7 +203,7 @@ inline void upload_sample_chunk(mkp_ctx* ctx, const PackedChunk& pc, uint32_t ti
     if (mkp_upload_chunk(ctx, &ch)) throw std::runtime_error(mkp_last_error(ctx));
 }
 
-// Fills hist[4][1025]; returns number of reads selected
+// Fills hist[4][MKP_HIST_BINS]; returns number of reads selected
 inline size_t sample_histogram(const BamReader& bam, mkp_ctx* ctx, const SamplerConfig& cfg, uint64_t* hist, uint64_t* inexact, std::vector<SampledChunk>* keep = nullptr) {
     int region_tid = -1;
     if (cfg.region) {
@@ -248,8 +248,8 @@ inline size_t sample_histogram(const BamReader& bam, mkp_ctx* ctx, const Sampler
     PackedChunk cand;
     std::vector<uint8_t> contributes, take;
     std::vector<uint32_t> fpos, fneg;
-    std::vector<uint64_t> batch_hist(4 * 1025);
-    memset(hist, 0, 4 * 1025 * sizeof(uint64_t));
+    std::vector<uint64_t> batch_hist(4 * MKP_HIST_BINS);
+    memset(hist, 0, 4 * MKP_HIST_BINS * sizeof(uint64_t));
     if (inexact) *inexact = 0;
 
     // One device pass decides which candidate reads contribute (MODE_HIST without a histogram); a second pass over the
@@ -278,15 +278,15 @@ inline size_t sample_histogram(const BamReader& bam, mkp_ctx* ctx, const Sampler
         contributes.assign(pc.recs.size(), 0);
         if (pc.recs.empty()) return;
         upload(pc, tid);
-        if (mkp_sample_histogram(ctx, cfg.include_unmapped ? 1 : 0, nullptr, nullptr, contributes.data(), nullptr)) throw std::runtime_error(mkp_last_error(ctx));
+        if (mkp_sample_histogram_wide(ctx, cfg.include_unmapped ? 1 : 0, nullptr, nullptr, contributes.data(), nullptr)) throw std::runtime_error(mkp_last_error(ctx));
     };
     auto add_selected = [&]() {       // histogram of the reads flagged in `take` (resident chunk)
         bool any = false;
         for (uint8_t t : take) any = any || t;
         if (!any) return;
         uint64_t inx = 0;
-        if (mkp_sample_histogram(ctx, cfg.include_unmapped ? 1 : 0, take.data(), batch_hist.data(), nullptr, &inx)) throw std::runtime_error(mkp_last_error(ctx));
-        for (int k = 0; k < 4 * 1025; k++) hist[k] += batch_hist[k];
+        if (mkp_sample_histogram_wide(ctx, cfg.include_unmapped ? 1 : 0, take.data(), batch_hist.data(), nullptr, &inx)) throw std::runtime_error(mkp_last_error(ctx));
+        for (int k = 0; k < 4 * MKP_HIST_BINS; k++) hist[k] += batch_hist[k];
         if (inexact) *inexact += inx;
     };
 
@@ -501,9 +501,9 @@ inline size_t sample_histogram_indexed(const BamReader& bam, mkp_ctx* ctx, const
         std::vector<uint64_t> load(std::max(1, coll.world), 0);
         for (auto& o : order) { int r = 0; for (int k = 1; k < coll.world; k++) if (load[k] < load[r]) r = k; owner[o.second] = r; load[r] += o.first + 1; }
     }
-    memset(hist, 0, 4 * 1025 * sizeof(uint64_t));
+    memset(hist, 0, 4 * MKP_HIST_BINS * sizeof(uint64_t));
     uint64_t inexact_local = 0, n_selected = 0;
-    std::vector<uint64_t> batch_hist(4 * 1025);
+    std::vector<uint64_t> batch_hist(4 * MKP_HIST_BINS);
     std::vector<uint32_t> fpos, fneg;
     double t_fetch = 0;
     const bool req_mapped = only_mapped || cfg.edge_on;
@@ -528,15 +528,15 @@ inline size_t sample_histogram_indexed(const BamReader& bam, mkp_ctx* ctx, const
         contributes->assign(pc.recs.size(), 0);
         if (pc.recs.empty()) return;
         upload(pc, tid);
-        if (mkp_sample_histogram(ctx, cfg.include_unmapped ? 1 : 0, nullptr, nullptr, contributes->data(), nullptr)) throw std::runtime_error(mkp_last_error(ctx));
+        if (mkp_sample_histogram_wide(ctx, cfg.include_unmapped ? 1 : 0, nullptr, nullptr, contributes->data(), nullptr)) throw std::runtime_error(mkp_last_error(ctx));
     };
     auto add_taken = [&](const std::vector<uint8_t>& take) {     // histogram of the flagged reads of the resident chunk
         bool any = false;
         for (uint8_t t : take) any = any || t;
         if (!any) return;
         uint64_t inx = 0;
-        if (mkp_sample_histogram(ctx, cfg.include_unmapped ? 1 : 0, take.data(), batch_hist.data(), nullptr, &inx)) throw std::runtime_error(mkp_last_error(ctx));
-        for (int k = 0; k < 4 * 1025; k++) hist[k] += batch_hist[k];
+        if (mkp_sample_histogram_wide(ctx, cfg.include_unmapped ? 1 : 0, take.data(), batch_hist.data(), nullptr, &inx)) throw std::runtime_error(mkp_last_error(ctx));
+        for (int k = 0; k < 4 * MKP_HIST_BINS; k++) hist[k] += batch_hist[k];
         inexact_local += inx;
     };
     auto key_of = [](const Grp& g) { return std::to_string(g.tid) + ":" + std::to_string(g.start) + "-" + std::to_string(g.end) + "/" + std::to_string(g.n); };
@@ -701,12 +701,12 @@ inline size_t sample_histogram_indexed(const BamReader& bam, mkp_ctx* ctx, const
     }
     // ---- the one exchange of a sharded run: sum of the histograms (+ the inexact-value count and the read count)
     if (coll.world > 1) {
-        std::vector<uint64_t> buf(4 * 1025 + 2);
-        memcpy(buf.data(), hist, 4 * 1025 * sizeof(uint64_t));
-        buf[4 * 1025] = inexact_local; buf[4 * 1025 + 1] = n_selected;
+        std::vector<uint64_t> buf(4 * MKP_HIST_BINS + 2);
+        memcpy(buf.data(), hist, 4 * MKP_HIST_BINS * sizeof(uint64_t));
+        buf[4 * MKP_HIST_BINS] = inexact_local; buf[4 * MKP_HIST_BINS + 1] = n_selected;
         coll.sum(buf.data(), buf.size());
-        memcpy(hist, buf.data(), 4 * 1025 * sizeof(uint64_t));
-        inexact_local = buf[4 * 1025]; n_selected = buf[4 * 1025 + 1];
+        memcpy(hist, buf.data(), 4 * MKP_HIST_BINS * sizeof(uint64_t));
+        inexact_local = buf[4 * MKP_HIST_BINS]; n_selected = buf[4 * MKP_HIST_BINS + 1];
     }
     if (inexact) *inexact = inexact_local;
     if (fetch_s) *fetch_s = t_fetch;
@@ -878,7 +878,7 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
         // ---- threshold estimation starts now when it can run beside the load: its candidates come straight from the file (host
         // fetch through the index), only its decode passes need the device and wait for `dev_ready`
         const bool estimate = o.filter_thresholds.empty() && !o.no_filtering;
-        std::vector<uint64_t> bg_hist(4 * 1025);
+        std::vector<uint64_t> bg_hist(4 * MKP_HIST_BINS);
         uint64_t bg_inexact = 0;
         double bg_fetch_s = 0;
         std::exception_ptr bg_err;
@@ -1031,9 +1031,9 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
             for (int b = 0; b < 4; b++) {
                 float thr;
                 uint64_t n = 0;
-                for (int k = 0; k <= 1024; k++) n += bg_hist[b * 1025 + k];
+                for (int k = 0; k < MKP_HIST_BINS; k++) n += bg_hist[b * MKP_HIST_BINS + k];
                 if (!n) continue;
-                if (!percentile_from_hist(bg_hist.data() + b * 1025, o.percentile, &thr)) throw std::runtime_error("not enough datapoints to estimate a threshold");
+                if (!percentile_from_hist(bg_hist.data() + b * MKP_HIST_BINS, o.percentile, &thr)) throw std::runtime_error("not enough datapoints to estimate a threshold");
                 P.base_threshold_set[b] = 1;
                 P.base_threshold[b] = thr;
                 if (!o.quiet && coll.rank == 0) fprintf(stderr, "> Using filter threshold %.9g for %c.\n", thr, "ACGT"[b]);
@@ -1050,7 +1050,7 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
             sc.include_unmapped = o.include_unmapped;
             sc.edge_on = P.edge_filter_on;
             sc.include = inc;
-            std::vector<uint64_t> hist(4 * 1025);
+            std::vector<uint64_t> hist(4 * MKP_HIST_BINS);
             uint64_t inexact = 0;
             if (bam.on_device && bam.have_index()) sample_histogram_indexed(bam, dev.ctx, sc, hist.data(), &inexact, coll, &fetch_s);
             else {
@@ -1061,9 +1061,9 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
             for (int b = 0; b < 4; b++) {
                 float thr;
                 uint64_t n = 0;
-                for (int k = 0; k <= 1024; k++) n += hist[b * 1025 + k];
+                for (int k = 0; k < MKP_HIST_BINS; k++) n += hist[b * MKP_HIST_BINS + k];
                 if (!n) continue;
-                if (!percentile_from_hist(hist.data() + b * 1025, o.percentile, &thr)) throw std::runtime_error("not enough datapoints to estimate a threshold");
+                if (!percentile_from_hist(hist.data() + b * MKP_HIST_BINS, o.percentile, &thr)) throw std::runtime_error("not enough datapoints to estimate a threshold");
                 P.base_threshold_set[b] = 1;
                 P.base_threshold[b] = thr;
                 if (!o.quiet && coll.rank == 0) fprintf(stderr, "> Using filter threshold %.9g for %c.\n", thr, "ACGT"[b]);
@@ -1575,9 +1575,10 @@ inline std::string f64_display(double v) {
     return std::string(buf, r.ptr);
 }
 
-// sampling + thresholds shared by both commands; fills the kept chunks when `keep` is given
+// sampling + thresholds shared by both commands; fills the kept chunks when `keep` is given. `inexact` receives the count of
+// sampled values off the histogram's 1/1024 grid: only a quantile of the histogram needs them on it
 inline void sample_for_summary(const SampleOptions& o, mkp_ctx* ctx, BamReader& bam, mkp_params* P, Region* region_out, bool* have_region, IncludeBed* include, bool* have_include,
-                               std::vector<uint64_t>* hist, std::vector<SampledChunk>* keep, size_t* n_selected) {
+                               std::vector<uint64_t>* hist, std::vector<SampledChunk>* keep, size_t* n_selected, uint64_t* inexact_out) {
     try { bam.open_device_index(o.in_bam, ctx); }
     catch (...) { throw; }
     if (!bam.have_index()) { bam = BamReader(); bam.open(o.in_bam, o.threads); }       // no index: the (small) file is read on the host
@@ -1609,11 +1610,15 @@ inline void sample_for_summary(const SampleOptions& o, mkp_ctx* ctx, BamReader& 
     sc.include_unmapped = !(o.only_mapped || *have_include);
     sc.edge_on = P->edge_filter_on;
     sc.include = *have_include ? include : nullptr;
-    hist->assign(4 * 1025, 0);
+    hist->assign(4 * MKP_HIST_BINS, 0);
     uint64_t inexact = 0;
     Collective solo;
     if (bam.on_device && bam.have_index()) *n_selected = sample_histogram_indexed(bam, ctx, sc, hist->data(), &inexact, solo, nullptr, keep);
     else *n_selected = sample_histogram(bam, ctx, sc, hist->data(), &inexact, keep);
+    *inexact_out = inexact;
+}
+
+inline void require_exact(uint64_t inexact) {
     if (inexact) throw std::runtime_error("sampled probabilities are not multiples of 1/1024 (" + std::to_string(inexact) + " values): exact quantiles impossible");
 }
 
@@ -1629,7 +1634,8 @@ inline int run_summary(const SampleOptions& o, std::string* text, std::string* e
         std::vector<uint64_t> hist;
         std::vector<SampledChunk> keep;
         size_t n_selected = 0;
-        sample_for_summary(o, dev.ctx, bam, &P, &region, &have_region, &include, &have_include, &hist, &keep, &n_selected);
+        uint64_t inexact = 0;
+        sample_for_summary(o, dev.ctx, bam, &P, &region, &have_region, &include, &have_include, &hist, &keep, &n_selected, &inexact);
         ModSummaryOut S;
         // thresholds (src/commands.rs:1086-1098, 1147-1160)
         for (auto& raw : o.mod_thresholds) {
@@ -1655,12 +1661,13 @@ inline int run_summary(const SampleOptions& o, std::string* text, std::string* e
                 }
             }
         } else if (!o.no_filtering) {
+            require_exact(inexact);
             for (int b = 0; b < 4; b++) {
                 uint64_t n = 0;
-                for (int k = 0; k <= 1024; k++) n += hist[b * 1025 + k];
+                for (int k = 0; k < MKP_HIST_BINS; k++) n += hist[b * MKP_HIST_BINS + k];
                 if (!n) continue;
                 float thr;
-                if (!percentile_from_hist(hist.data() + b * 1025, o.percentile, &thr)) throw std::runtime_error("not enough datapoints to estimate a threshold");
+                if (!percentile_from_hist(hist.data() + b * MKP_HIST_BINS, o.percentile, &thr)) throw std::runtime_error("not enough datapoints to estimate a threshold");
                 P.base_threshold_set[b] = 1; P.base_threshold[b] = thr;
             }
         }
@@ -1766,16 +1773,18 @@ inline int run_sample_probs(const SampleOptions& o, std::string* text, std::stri
         IncludeBed include; bool have_include = false;
         std::vector<uint64_t> hist;
         size_t n_selected = 0;
-        sample_for_summary(o, dev.ctx, bam, &P, &region, &have_region, &include, &have_include, &hist, nullptr, &n_selected);
+        uint64_t inexact = 0;
+        sample_for_summary(o, dev.ctx, bam, &P, &region, &have_region, &include, &have_include, &hist, nullptr, &n_selected, &inexact);
+        require_exact(inexact);
         std::vector<std::vector<std::string>> rows;
         rows.push_back({"base", "percentile", "threshold"});
         for (int b = 0; b < 4; b++) {
             uint64_t n = 0;
-            for (int k = 0; k <= 1024; k++) n += hist[b * 1025 + k];
+            for (int k = 0; k < MKP_HIST_BINS; k++) n += hist[b * MKP_HIST_BINS + k];
             if (!n) continue;
             for (float q : qs) {
                 float v;
-                if (!percentile_from_hist(hist.data() + b * 1025, q, &v)) throw std::runtime_error("not enough datapoints to calculate percentiles");
+                if (!percentile_from_hist(hist.data() + b * MKP_HIST_BINS, q, &v)) throw std::runtime_error("not enough datapoints to calculate percentiles");
                 volatile float pct = q * 100.0f;
                 rows.push_back({std::string(1, "ACGT"[b]), f32_display(pct), f32_display(v)});
             }

@@ -774,7 +774,7 @@ static int sample_decode(mkp_ctx* ctx, int include_unaligned, const uint8_t* tak
         C.take = ctx->d_take.as<uint8_t>();
     }
     if (out_words) {
-        CK(ctx->d_hist.ensure(std::max<size_t>(4 * 1025, out_words) * 8));     // one size for both uses: no regrowth between them
+        CK(ctx->d_hist.ensure(std::max<size_t>(4 * MKP_HIST_BINS, out_words) * 8));     // one size for both uses: no regrowth between them
         CK(cudaMemsetAsync(ctx->d_hist.p, 0, out_words * 8, st));
         if (summary) C.summ = ctx->d_hist.as<unsigned long long>();
         else C.hist = ctx->d_hist.as<unsigned long long>();
@@ -782,10 +782,10 @@ static int sample_decode(mkp_ctx* ctx, int include_unaligned, const uint8_t* tak
     return decode(ctx, C, grid);
 }
 
-int mkp_sample_histogram(mkp_ctx* ctx, int include_unaligned, const uint8_t* take, uint64_t* hist, uint8_t* contributes, uint64_t* inexact) {
+int mkp_sample_histogram_wide(mkp_ctx* ctx, int include_unaligned, const uint8_t* take, uint64_t* hist, uint8_t* contributes, uint64_t* inexact) {
     if (!ctx) return -1;
-    if (int rc = sample_decode(ctx, include_unaligned, take, false, hist ? 4 * 1025 : 0)) return rc;
-    if (hist) CK(cudaMemcpyAsync(hist, ctx->d_hist.p, 4 * 1025 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    if (int rc = sample_decode(ctx, include_unaligned, take, false, hist ? 4 * MKP_HIST_BINS : 0)) return rc;
+    if (hist) CK(cudaMemcpyAsync(hist, ctx->d_hist.p, 4 * MKP_HIST_BINS * 8, cudaMemcpyDeviceToHost, ctx->stream));
     std::vector<ReadMeta> metas;
     if (contributes) {
         metas.resize(ctx->n_reads);
@@ -795,6 +795,19 @@ int mkp_sample_histogram(mkp_ctx* ctx, int include_unaligned, const uint8_t* tak
     if (int rc = finish_status(ctx, nullptr, &h)) return rc;
     if (contributes) for (uint32_t i = 0; i < ctx->n_reads; i++) contributes[i] = metas[i].n_hist > 0;
     if (inexact) *inexact = h.hist_inexact;
+    return 0;
+}
+
+// u64[4][1025]: values above 1.0 go to bin 1024 and count as inexact
+int mkp_sample_histogram(mkp_ctx* ctx, int include_unaligned, const uint8_t* take, uint64_t* hist, uint8_t* contributes, uint64_t* inexact) {
+    std::vector<uint64_t> wide(hist ? 4 * MKP_HIST_BINS : 0);
+    uint64_t inx = 0;
+    if (int rc = mkp_sample_histogram_wide(ctx, include_unaligned, take, hist ? wide.data() : nullptr, contributes, &inx)) return rc;
+    for (int b = 0; hist && b < 4; b++) {
+        memcpy(hist + b * 1025, wide.data() + b * MKP_HIST_BINS, 1025 * 8);
+        for (int k = 1025; k < MKP_HIST_BINS; k++) { hist[b * 1025 + 1024] += wide[b * MKP_HIST_BINS + k]; inx += wide[b * MKP_HIST_BINS + k]; }
+    }
+    if (inexact) *inexact = inx;
     return 0;
 }
 

@@ -92,7 +92,7 @@ struct ChunkDev {
     uint32_t* scr_cq; uint32_t* scr_cr;
     uint32_t max_ncigar, max_blocks;
     // sampling
-    unsigned long long* hist;   // [4][1025]
+    unsigned long long* hist;   // [4][MKP_HIST_BINS]
     unsigned long long* hist_inexact;
     const uint8_t* take;
     uint32_t hist_include_unaligned;
@@ -1394,12 +1394,13 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                     } else {
                         uint32_t hm = __ballot_sync(FULL, hist_ok);
                         if (hist_ok) {
-                            // stash (bin | base<<16 | inexact<<20) in the call buffer; committed after validation
+                            // stash (bin | base<<16 | inexact<<20) in the call buffer; committed after validation. Values
+                            // above 1.0 are legal (ML sums up to 1.01, ReDistribute shares) and get their own bins
                             float sc = __fmul_rn(C.summ ? 0.f : hist_v, 1024.0f);
                             int bin = (int)rintf(sc);
-                            uint32_t inexact = ((float)bin != sc || bin < 0 || bin > 1024) ? 1u : 0u;
+                            uint32_t inexact = ((float)bin != sc || bin < 0 || bin >= MKP_HIST_BINS) ? 1u : 0u;
                             if (bin < 0) bin = 0;
-                            if (bin > 1024) bin = 1024;
+                            if (bin >= MKP_HIST_BINS) bin = MKP_HIST_BINS - 1;
                             calls[n_hist + __popc(hm & ((1u << lane) - 1u))] = make_uint2((uint32_t)bin | ((uint32_t)hist_base << 16) | (inexact << 20), __float_as_uint(hist_v));
                         }
                         n_hist += __popc(hm);
@@ -1564,12 +1565,12 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                 if (C.hist) {
                     for (uint32_t k = lane; k < n_hist; k += 32) {
                         uint32_t v = calls[k].x;
-                        atomicAdd(&C.hist[((v >> 16) & 3u) * 1025u + (v & 0xffffu)], 1ull);
+                        atomicAdd(&C.hist[((v >> 16) & 3u) * MKP_HIST_BINS + (v & 0xffffu)], 1ull);
                         if ((v >> 20) & 1u) atomicAdd(C.hist_inexact, 1ull);
                     }
                     if (lane == 0) for (int sb = 0; sb < 8; sb++) if (imp_hist[sb]) {
                         const int tb = (sb >> 2) == 0 ? (sb & 3) : 3 - (sb & 3);
-                        atomicAdd(&C.hist[tb * 1025u + 1024u], imp_hist[sb]);
+                        atomicAdd(&C.hist[tb * MKP_HIST_BINS + 1024u], imp_hist[sb]);
                     }
                 }
             }
