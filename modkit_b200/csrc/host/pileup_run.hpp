@@ -13,6 +13,7 @@
 #include <future>
 #include <memory>
 #include <filesystem>
+#include <optional>
 #include <set>
 #include <unordered_set>
 
@@ -161,10 +162,10 @@ inline void trace_mark0(const char* what) { trace_clock().mark(0, what); }
 struct SamplerConfig {
     int threads = 4;
     int workers = 4;                   // host threads that fetch candidates (not part of the schedule)
-    std::shared_ptr<void>* defer_free = nullptr;         // indexed sampler: its candidate buffers (hundreds of MB) are handed over instead of being
-                                                         // released before the result is returned; the caller drops them when convenient
-    std::shared_future<void>* device_ready = nullptr;    // indexed sampler: the candidates are fetched from the file first (host only); the
-                                                         // decode passes wait for this (the device is busy loading the BAM until then)
+    std::shared_ptr<void>* defer_free = nullptr;         // the candidate buffers (hundreds of MB with an index) are handed over instead of
+                                                         // being released before the result is returned; the caller drops them when convenient
+    std::shared_future<void>* device_ready = nullptr;    // the candidates are fetched first (host only); the decode passes wait for this
+                                                         // (the device is busy loading the BAM until then)
     uint32_t sampling_interval_size = 1000000;
     bool take_all = false;
     size_t num_reads = 10042;
@@ -172,6 +173,7 @@ struct SamplerConfig {
     bool include_unmapped = false;
     bool edge_on = false;
     const IncludeBed* include = nullptr;
+    bool keep = false;                 // also return the sampled reads (summary's second pass); needs host-packed reads, so not the device-resident source
 };
 
 inline bool sampler_flag_ok(const RecRef& r, bool require_mapped) {
@@ -185,207 +187,81 @@ inline bool sampler_flag_ok(const RecRef& r, bool require_mapped) {
 // the sampled reads themselves (summary: a second device pass over them once the thresholds are known)
 struct SampledChunk { PackedChunk pc; std::vector<uint8_t> take; uint32_t tid = 0; };
 
-// resident chunk of sampled reads: without coordinates of its own, except with --include-bed (bitmaps of the contig)
-inline void upload_sample_chunk(mkp_ctx* ctx, const PackedChunk& pc, uint32_t tid, const IncludeBed* include, std::vector<uint32_t>* fpos, std::vector<uint32_t>* fneg) {
+struct SampleResult {
+    std::vector<uint64_t> hist = std::vector<uint64_t>(4 * MKP_HIST_BINS, 0);    // [4][MKP_HIST_BINS], summed over the ranks
+    uint64_t inexact = 0;              // sampled values off the 1/1024 grid
+    size_t n_selected = 0;             // reads selected, all ranks
+    double fetch_s = 0;                // host fetch + pack of the planned candidates
+    std::vector<SampledChunk> keep;    // SamplerConfig::keep: the selected reads, flagged in `take` of their chunks
+};
+
+// Candidate reads of one sampling group (tid < 0: the reads without coordinates) in file order, from one of three sources:
+// the index fetch (the reader has a BAI, BamReader::fetch_*: the record bytes come from the file), the records the reader holds
+// on the host, or the records it holds on the device (only listed; sliced on the GPU when the chunk is uploaded). A resident
+// reader is never loaded range by range (that needs the index), so its records need no ensure_tid.
+struct Candidates {
+    const BamReader& bam;
+    const bool req_mapped;
+    BamReader::FetchCursor fc;         // index source
+    std::vector<RecRef> recs, got;     // resident sources: the group's candidates, `next` the first not handed out
+    size_t next = 0;
+    bool done = false;
+    Candidates(const BamReader& b, int64_t tid, uint32_t start, uint32_t end, bool req_mapped_) : bam(b), req_mapped(req_mapped_) {
+        if (bam.have_index()) { fc = tid < 0 ? bam.fetch_unplaced_begin() : bam.fetch_begin((uint32_t)tid, start, end); done = fc.done; return; }
+        auto add = [&](const RecRef& r) { if (sampler_flag_ok(r, req_mapped)) recs.push_back(r); };
+        if (tid < 0) for (auto& r : bam.unplaced) add(r);
+        else bam.for_overlapping((uint32_t)tid, start, end, add);
+        done = recs.empty();
+    }
+    // appends up to n more candidates to `out` (packed unless the records are on the device)
+    void more(size_t n, PackedChunk* out) {
+        if (bam.have_index()) {
+            got.clear();
+            bam.fetch_more(fc, n, [&](const RecRef& r) { return sampler_flag_ok(r, req_mapped); }, &got);
+            for (auto& r : got) { pack_record(fc.bytes(r), r.size, out); out->recs.push_back(r); }     // (bytes valid until the next fetch_more)
+            done = fc.done;
+            return;
+        }
+        for (const size_t stop = next + std::min(n, recs.size() - next); next < stop; next++) {
+            if (!bam.on_device) pack_record(bam.rec(recs[next]), recs[next].size, out);
+            out->recs.push_back(recs[next]);
+        }
+        done = next == recs.size();
+    }
+};
+
+// Makes a chunk of sampled reads the resident chunk: packed reads are uploaded, device-resident ones sliced on the GPU. The chunk
+// has no coordinates of its own, except with --include-bed: then it spans its reads and carries the bitmaps of contig `tid`.
+inline void upload_sampled(const BamReader& bam, mkp_ctx* ctx, const PackedChunk& pc, uint32_t tid, const IncludeBed* include) {
     mkp_chunk ch;
     memset(&ch, 0, sizeof ch);
     ch.start = 0; ch.end = 32;
+    std::vector<uint32_t> fpos, fneg;
     if (include) {
         int64_t lo = INT64_MAX, hi = 0;
         for (auto& r : pc.recs) { lo = std::min<int64_t>(lo, r.pos); hi = std::max<int64_t>(hi, r.end); }
         if (lo < 0) lo = 0;
         if (hi <= lo) hi = lo + 1;
         ch.start = (uint32_t)lo; ch.end = (uint32_t)hi;
-        include->bitmaps(tid, ch.start, ch.end, fpos, fneg);
-        ch.focus_pos = fpos->data(); ch.focus_neg = fneg->data();
+        include->bitmaps(tid, ch.start, ch.end, &fpos, &fneg);
+        ch.focus_pos = fpos.data(); ch.focus_neg = fneg.data();
     }
+    if (bam.on_device && !bam.have_index()) { device_chunk(bam, pc.recs, ch.start, ch.end, ch.focus_pos, ch.focus_neg); return; }
     ch.hdrs = pc.hdrs.data(); ch.n_reads = (uint32_t)pc.hdrs.size(); ch.heap = pc.heap.data(); ch.heap_bytes = pc.heap.size();
     if (mkp_upload_chunk(ctx, &ch)) throw std::runtime_error(mkp_last_error(ctx));
 }
 
-// Fills hist[4][MKP_HIST_BINS]; returns number of reads selected
-inline size_t sample_histogram(const BamReader& bam, mkp_ctx* ctx, const SamplerConfig& cfg, uint64_t* hist, uint64_t* inexact, std::vector<SampledChunk>* keep = nullptr) {
-    int region_tid = -1;
-    if (cfg.region) {
-        for (size_t i = 0; i < bam.ref_names.size(); i++) if (bam.ref_names[i] == cfg.region->name) region_tid = (int)i;
-        if (region_tid < 0) throw std::runtime_error("did not find target_id for region in header");
+// The schedule's unit of selection: the first `limit` contributing reads of recs[lo, hi) count towards the group (`used`); those
+// not selected by an earlier group of the contig are flagged in `take`.
+inline void select_first(const std::vector<RecRef>& recs, const std::vector<uint8_t>& contributes, size_t lo, size_t hi, size_t limit, size_t* used,
+                         std::unordered_set<uint64_t>* selected, std::vector<uint8_t>* take) {
+    for (size_t k = lo; k < hi && *used < limit; k++) {
+        if (!contributes[k]) continue;
+        ++*used;
+        if (selected->insert(recs[k].off).second) (*take)[k] = 1;
     }
-    uint64_t total_mapped = 0, total_unmapped = 0;
-    std::map<uint32_t, uint64_t> mapped;
-    for (uint32_t t = 0; t < bam.ref_names.size(); t++) {
-        if (cfg.region && (int)t != region_tid) continue;
-        if (!cfg.region && cfg.include && !cfg.include->has_contig(t)) continue;
-        mapped[t] = bam.stats.n_mapped[t];
-        total_mapped += bam.stats.n_mapped[t];
-        total_unmapped += bam.stats.n_unmapped[t];
-    }
-    if (!cfg.region) total_unmapped += bam.stats.n_no_coor;
-    const uint64_t total = cfg.include_unmapped ? total_mapped + total_unmapped : total_mapped;
-    if (!total) throw std::runtime_error("zero reads found in bam index");
-    std::map<uint32_t, int64_t> quota;   // -1 = all
-    for (auto& kv : mapped) {
-        if (!kv.second) continue;
-        if (cfg.take_all) { quota[kv.first] = -1; continue; }
-        const float frac = (float)kv.second / (float)total;
-        quota[kv.first] = (int64_t)std::min<uint64_t>((uint64_t)std::ceil((float)cfg.num_reads * frac), kv.second);
-    }
-    std::vector<RefTarget> contigs;
-    std::map<uint32_t, uint32_t> contig_len;
-    for (uint32_t t = 0; t < bam.ref_names.size(); t++) {
-        if (!quota.count(t)) continue;
-        RefTarget c{t, 0, bam.ref_lens[t], bam.ref_names[t]};
-        if (cfg.region) { c.start = cfg.region->start; c.length = cfg.region->end - cfg.region->start; }
-        contigs.push_back(c);
-        contig_len[t] = c.length;
-    }
-    std::vector<std::vector<size_t>> groups;
-    std::vector<RefInterval> ivs;
-    if (!contigs.empty()) ivs = reference_intervals(contigs, cfg.sampling_interval_size, false, nullptr, &groups);
-    const size_t B = std::max<size_t>(1, (size_t)std::floor((float)cfg.threads * 1.5f));
-    const bool only_mapped = !cfg.include_unmapped;
-    std::map<uint32_t, size_t> so_far;
-    std::unordered_set<uint64_t> selected_ids;     // record identity = offset in the stream
-    PackedChunk cand;
-    std::vector<uint8_t> contributes, take;
-    std::vector<uint32_t> fpos, fneg;
-    std::vector<uint64_t> batch_hist(4 * MKP_HIST_BINS);
-    memset(hist, 0, 4 * MKP_HIST_BINS * sizeof(uint64_t));
-    if (inexact) *inexact = 0;
-
-    // One device pass decides which candidate reads contribute (MODE_HIST without a histogram); a second pass over the
-    // same resident chunk adds the values of the newly selected reads to the histogram.
-    auto upload = [&](PackedChunk& pc, uint32_t tid) {
-        mkp_chunk ch;
-        memset(&ch, 0, sizeof ch);
-        ch.start = 0; ch.end = 32;
-        if (cfg.include) {
-            // chunk range = span of the candidates, bitmaps = the include-bed of this contig
-            int64_t lo = INT64_MAX, hi = 0;
-            for (auto& r : pc.recs) { lo = std::min<int64_t>(lo, r.pos); hi = std::max<int64_t>(hi, r.end); }
-            if (lo < 0) lo = 0;
-            if (hi <= lo) hi = lo + 1;
-            ch.start = (uint32_t)lo; ch.end = (uint32_t)hi;
-            cfg.include->bitmaps(tid, ch.start, ch.end, &fpos, &fneg);
-            ch.focus_pos = fpos.data(); ch.focus_neg = fneg.data();
-        }
-        if (bam.on_device) { device_chunk(bam, pc.recs, ch.start, ch.end, ch.focus_pos, ch.focus_neg); return; }
-        ch.hdrs = pc.hdrs.data(); ch.n_reads = (uint32_t)pc.hdrs.size(); ch.heap = pc.heap.data(); ch.heap_bytes = pc.heap.size();
-        if (mkp_upload_chunk(ctx, &ch)) throw std::runtime_error(mkp_last_error(ctx));
-    };
-    // candidate records: sliced on the host (pack_record) or, with the device ingest, only listed (sliced on the GPU)
-    auto add_candidate = [&](const RecRef& r) { if (!bam.on_device) pack_record(bam.rec(r), r.size, &cand); cand.recs.push_back(r); };
-    auto decode_contributes = [&](PackedChunk& pc, uint32_t tid) {
-        contributes.assign(pc.recs.size(), 0);
-        if (pc.recs.empty()) return;
-        upload(pc, tid);
-        if (mkp_sample_histogram_wide(ctx, cfg.include_unmapped ? 1 : 0, nullptr, nullptr, contributes.data(), nullptr)) throw std::runtime_error(mkp_last_error(ctx));
-    };
-    auto add_selected = [&]() {       // histogram of the reads flagged in `take` (resident chunk)
-        bool any = false;
-        for (uint8_t t : take) any = any || t;
-        if (!any) return;
-        uint64_t inx = 0;
-        if (mkp_sample_histogram_wide(ctx, cfg.include_unmapped ? 1 : 0, take.data(), batch_hist.data(), nullptr, &inx)) throw std::runtime_error(mkp_last_error(ctx));
-        for (int k = 0; k < 4 * MKP_HIST_BINS; k++) hist[k] += batch_hist[k];
-        if (inexact) *inexact += inx;
-    };
-
-    struct Grp { uint32_t tid, start, end; int64_t n; };
-    for (size_t sb = 0; sb < groups.size(); sb += B) {
-        std::vector<size_t> coords;
-        for (size_t k = sb; k < std::min(groups.size(), sb + B); k++) for (size_t i : groups[k]) coords.push_back(i);
-        std::sort(coords.begin(), coords.end(), [&](size_t a, size_t b) { return ivs[a].tid != ivs[b].tid ? ivs[a].tid < ivs[b].tid : ivs[a].start < ivs[b].start; });
-        std::map<uint32_t, uint32_t> len_c;
-        for (size_t i : coords) len_c[ivs[i].tid] += ivs[i].end - ivs[i].start;
-        std::map<uint32_t, int64_t> k_c;
-        for (auto& kv : len_c) {
-            auto q = quota.find(kv.first);
-            if (q == quota.end()) continue;
-            if (q->second < 0) { k_c[kv.first] = -1; continue; }
-            const size_t done = so_far.count(kv.first) ? so_far[kv.first] : 0;
-            if ((size_t)q->second <= done) continue;
-            const float f = (float)kv.second / (float)contig_len[kv.first];
-            k_c[kv.first] = (int64_t)std::ceil(f * (float)((size_t)q->second - done));
-        }
-        std::vector<Grp> todo;
-        bool have = false;
-        Grp slack{};
-        for (size_t i : coords) {
-            const RefInterval& iv = ivs[i];
-            auto kc = k_c.find(iv.tid);
-            if (kc == k_c.end()) continue;
-            if (kc->second < 0) { todo.push_back({iv.tid, iv.start, iv.end, -1}); continue; }
-            const float f = (float)(iv.end - iv.start) / (float)len_c[iv.tid];
-            const int64_t x = (int64_t)std::ceil((float)kc->second * f);
-            Grp cur{iv.tid, iv.start, iv.end, x};
-            if (x < 50) {
-                if (!have) { slack = cur; have = true; }
-                else if (slack.tid == cur.tid) {
-                    Grp m{cur.tid, std::min(slack.start, cur.start), std::max(slack.end, cur.end), slack.n + x};
-                    if (m.n < 50) slack = m; else { todo.push_back(m); have = false; }
-                } else { todo.push_back(slack); slack = cur; }
-            } else if (have) {
-                have = false;
-                if (slack.tid == cur.tid) todo.push_back({cur.tid, std::min(slack.start, cur.start), std::max(slack.end, cur.end), slack.n + x});
-                else { todo.push_back(slack); todo.push_back(cur); }
-            } else todo.push_back(cur);
-        }
-        if (have) todo.push_back(slack);
-        // candidates of one interval at a time: first n contributing records in file order; extend while short
-        for (const Grp& g : todo) {
-            if (cfg.include && !cfg.include->overlaps_any(g.tid, g.start, g.end)) continue;
-            std::vector<RecRef> recs;
-            bam.ensure_tid(g.tid);          // ranged device ingest: the contig's byte range becomes resident
-            bam.for_overlapping(g.tid, g.start, g.end, [&](const RecRef& r) { if (sampler_flag_ok(r, only_mapped || cfg.edge_on)) recs.push_back(r); });
-            size_t used = 0, cursor = 0;
-            while (cursor < recs.size() && (g.n < 0 || used < (size_t)g.n)) {
-                const size_t want = g.n < 0 ? recs.size() : std::min(recs.size(), cursor + (size_t)(g.n - (int64_t)used) * 2 + 32);
-                cand.clear();
-                for (size_t k = cursor; k < want; k++) add_candidate(recs[k]);
-                decode_contributes(cand, g.tid);
-                take.assign(cand.recs.size(), 0);
-                for (size_t k = 0; k < cand.recs.size() && (g.n < 0 || used < (size_t)g.n); k++) {
-                    if (!contributes[k]) continue;
-                    used++;
-                    if (selected_ids.insert(cand.recs[k].off).second) take[k] = 1;
-                }
-                add_selected();
-                if (keep && !bam.on_device) { bool any = false; for (uint8_t x : take) any = any || x; if (any) keep->push_back({cand, take, g.tid}); }
-                cursor = want;
-            }
-            so_far[g.tid] += used;
-        }
-    }
-    if (!only_mapped) {   // reads without coordinates (reads_sampler/mod.rs:85-129)
-        const size_t limit = cfg.take_all ? (size_t)-1 : (cfg.num_reads > selected_ids.size() ? cfg.num_reads - selected_ids.size() : 0);
-        cand.clear();
-        bam.ensure_unplaced();
-        for (auto& r : bam.unplaced) if (sampler_flag_ok(r, cfg.edge_on)) add_candidate(r);
-        if (!cand.recs.empty()) {
-            decode_contributes(cand, 0);
-            take.assign(cand.recs.size(), 0);
-            size_t used = 0;
-            for (size_t k = 0; k < cand.recs.size() && used < limit; k++) {
-                if (!contributes[k]) continue;
-                used++;
-                if (selected_ids.insert(cand.recs[k].off).second) take[k] = 1;
-            }
-            add_selected();
-            if (keep && !bam.on_device) keep->push_back({cand, take, 0});
-        }
-    }
-    return selected_ids.size();
 }
 
-// ---- the same schedule on an indexed file, without the per-group device round trips -----------------------------
-// The candidates come straight from the file (BamReader::fetch_*: BAI linear index + zlib on the few members that hold
-// them), so the sampler does not depend on what is resident on the device, and the per-contig state of the schedule
-// (`so_far`) makes contigs independent: in an interval-sharded run every rank samples the contigs it owns and the
-// histograms are summed once (SURVEY 8e). Per contig the schedule is first simulated under the assumption that every group
-// finds its quota (true whenever the coverage is not tiny); the candidates of all planned groups are fetched in parallel,
-// decoded in ONE device pass, and the real schedule then consumes them in order. A group that deviates from the plan, or
-// needs more candidates than were fetched, falls back to fetching and decoding on demand - the result is the same reads
-// either way: the first n contributing records of every group, in file order.
 struct Collective {          // sum over the ranks of a sharded run (in place); world == 1: nothing to do
     int rank = 0, world = 1;
     int (*allreduce_sum)(uint64_t* buf, size_t n, void* user) = nullptr;
@@ -404,9 +280,18 @@ inline void append_packed(const PackedChunk& src, PackedChunk* dst) {
     dst->recs.insert(dst->recs.end(), src.recs.begin(), src.recs.end());
 }
 
-inline size_t sample_histogram_indexed(const BamReader& bam, mkp_ctx* ctx, const SamplerConfig& cfg, uint64_t* hist, uint64_t* inexact,
-                                       const Collective& coll, double* fetch_s = nullptr, std::vector<SampledChunk>* keep = nullptr) {
+// The sampling schedule of the reference (reads_sampler/sampling_schedule.rs:171-615) and the histogram of the reads it selects:
+// the first n contributing records of every group, in file order. The schedule's state is per contig (`done`, the reads
+// selected so far), and the records of different contigs are disjoint, so walking contig by contig gives the same groups and
+// the same reads as the reference's walk over super-batches of all contigs (oracle/driver.hpp:427-500): a slack group never
+// spans two contigs. The contigs are therefore independent: in an interval-sharded run every rank samples the contigs it owns
+// and the histograms are summed once (SURVEY 8e). Per contig the schedule is first simulated under the assumption that every
+// group finds its quota (true whenever the coverage is not tiny); the candidates of all planned groups are fetched in parallel,
+// decoded in ONE device pass, and the real schedule then consumes them in order. A group that deviates from the plan, or needs
+// more candidates than were fetched, fetches and decodes on demand - the reads are the same either way.
+inline SampleResult sample_histogram(const BamReader& bam, mkp_ctx* ctx, const SamplerConfig& cfg, const Collective& coll = Collective()) {
     using clk = std::chrono::steady_clock;
+    if (coll.world > 1 && !bam.have_index()) throw std::runtime_error("interval-sharded runs need a BAM index (.bai)");
     int region_tid = -1;
     if (cfg.region) {
         for (size_t i = 0; i < bam.ref_names.size(); i++) if (bam.ref_names[i] == cfg.region->name) region_tid = (int)i;
@@ -444,7 +329,6 @@ inline size_t sample_histogram_indexed(const BamReader& bam, mkp_ctx* ctx, const
     std::vector<RefInterval> ivs;
     if (!contigs.empty()) ivs = reference_intervals(contigs, cfg.sampling_interval_size, false, nullptr, &groups);
     const size_t B = std::max<size_t>(1, (size_t)std::floor((float)cfg.threads * 1.5f));
-    const bool only_mapped = !cfg.include_unmapped;
     // super-batch structure: per super-batch and contig, the contig's intervals (position order) and their total length
     struct SbC { std::vector<size_t> iv; uint32_t len = 0; };
     std::vector<std::map<uint32_t, SbC>> sbs;
@@ -457,7 +341,7 @@ inline size_t sample_histogram_indexed(const BamReader& bam, mkp_ctx* ctx, const
         sbs.push_back(std::move(m));
     }
     struct Grp { uint32_t tid, start, end; int64_t n; };
-    // groups of contig t in super-batch s given the reads sampled from the contig so far (sampling_schedule.rs:171-615)
+    // groups of contig t in super-batch s given the reads sampled from the contig so far; groups of fewer than 50 reads merge
     auto todo_for = [&](size_t s, uint32_t t, size_t done) {
         std::vector<Grp> todo;
         auto sc = sbs[s].find(t);
@@ -501,47 +385,30 @@ inline size_t sample_histogram_indexed(const BamReader& bam, mkp_ctx* ctx, const
         std::vector<uint64_t> load(std::max(1, coll.world), 0);
         for (auto& o : order) { int r = 0; for (int k = 1; k < coll.world; k++) if (load[k] < load[r]) r = k; owner[o.second] = r; load[r] += o.first + 1; }
     }
-    memset(hist, 0, 4 * MKP_HIST_BINS * sizeof(uint64_t));
-    uint64_t inexact_local = 0, n_selected = 0;
+    SampleResult res;
     std::vector<uint64_t> batch_hist(4 * MKP_HIST_BINS);
-    std::vector<uint32_t> fpos, fneg;
-    double t_fetch = 0;
-    const bool req_mapped = only_mapped || cfg.edge_on;
+    const bool req_mapped = !cfg.include_unmapped || cfg.edge_on;
 
-    auto upload = [&](PackedChunk& pc, uint32_t tid) {
-        mkp_chunk ch;
-        memset(&ch, 0, sizeof ch);
-        ch.start = 0; ch.end = 32;
-        if (cfg.include) {
-            int64_t lo = INT64_MAX, hi = 0;
-            for (auto& r : pc.recs) { lo = std::min<int64_t>(lo, r.pos); hi = std::max<int64_t>(hi, r.end); }
-            if (lo < 0) lo = 0;
-            if (hi <= lo) hi = lo + 1;
-            ch.start = (uint32_t)lo; ch.end = (uint32_t)hi;
-            cfg.include->bitmaps(tid, ch.start, ch.end, &fpos, &fneg);
-            ch.focus_pos = fpos.data(); ch.focus_neg = fneg.data();
-        }
-        ch.hdrs = pc.hdrs.data(); ch.n_reads = (uint32_t)pc.hdrs.size(); ch.heap = pc.heap.data(); ch.heap_bytes = pc.heap.size();
-        if (mkp_upload_chunk(ctx, &ch)) throw std::runtime_error(mkp_last_error(ctx));
-    };
-    auto contributes_of = [&](PackedChunk& pc, uint32_t tid, std::vector<uint8_t>* contributes) {
+    // one device pass decides which reads of a chunk contribute (MODE_HIST without a histogram); a second pass over the same
+    // resident chunk adds the values of the selected reads to the histogram
+    auto decode = [&](const PackedChunk& pc, uint32_t tid, std::vector<uint8_t>* contributes) {
         contributes->assign(pc.recs.size(), 0);
         if (pc.recs.empty()) return;
-        upload(pc, tid);
+        upload_sampled(bam, ctx, pc, tid, cfg.include);
         if (mkp_sample_histogram_wide(ctx, cfg.include_unmapped ? 1 : 0, nullptr, nullptr, contributes->data(), nullptr)) throw std::runtime_error(mkp_last_error(ctx));
     };
+    auto any = [](const std::vector<uint8_t>& take) { for (uint8_t t : take) if (t) return true; return false; };
     auto add_taken = [&](const std::vector<uint8_t>& take) {     // histogram of the flagged reads of the resident chunk
-        bool any = false;
-        for (uint8_t t : take) any = any || t;
-        if (!any) return;
+        if (!any(take)) return;
         uint64_t inx = 0;
         if (mkp_sample_histogram_wide(ctx, cfg.include_unmapped ? 1 : 0, take.data(), batch_hist.data(), nullptr, &inx)) throw std::runtime_error(mkp_last_error(ctx));
-        for (int k = 0; k < 4 * MKP_HIST_BINS; k++) hist[k] += batch_hist[k];
-        inexact_local += inx;
+        for (int k = 0; k < 4 * MKP_HIST_BINS; k++) res.hist[k] += batch_hist[k];
+        res.inexact += inx;
     };
+    auto keep = [&](PackedChunk&& pc, std::vector<uint8_t>&& take, uint32_t tid) { if (cfg.keep && any(take)) res.keep.push_back({std::move(pc), std::move(take), tid}); };
     auto key_of = [](const Grp& g) { return std::to_string(g.tid) + ":" + std::to_string(g.start) + "-" + std::to_string(g.end) + "/" + std::to_string(g.n); };
 
-    struct Planned { Grp g; BamReader::FetchCursor cur; PackedChunk pc; size_t lo = 0, hi = 0; bool used = false; };
+    struct Planned { Grp g; std::optional<Candidates> cur; PackedChunk pc; size_t lo = 0, hi = 0; bool used = false; };
     struct ContigPlan { uint32_t tid = 0; std::vector<Planned> plan; size_t bulk = 0; };
     struct Bulk { PackedChunk pc; std::vector<uint8_t> contributes, take; uint32_t tid = 0; };
     struct Heavy { std::vector<ContigPlan> cps; std::vector<Bulk> bulks; };
@@ -556,12 +423,13 @@ inline size_t sample_histogram_indexed(const BamReader& bam, mkp_ctx* ctx, const
         size_t done = 0;
         for (size_t s = 0; s < sbs.size(); s++) for (const Grp& g : todo_for(s, t, done)) {
             if (cfg.include && !cfg.include->overlaps_any(g.tid, g.start, g.end)) continue;
-            Planned p; p.g = g; cp.plan.push_back(std::move(p));
+            cp.plan.emplace_back();
+            cp.plan.back().g = g;
             if (g.n >= 0) done += (size_t)g.n;
         }
         cps.push_back(std::move(cp));
     }
-    // ---- fetch the candidates of all planned groups of all contigs (parallel over groups)
+    // ---- fetch the candidates of all planned groups of all contigs (parallel over groups; a copy of RecRefs when resident)
     const auto tf0 = clk::now();
     {
         std::vector<Planned*> all;
@@ -571,19 +439,13 @@ inline size_t sample_histogram_indexed(const BamReader& bam, mkp_ctx* ctx, const
         std::mutex mu;
         auto work = [&]() {
             try {
-                std::vector<RecRef> recs;
                 for (;;) {
                     const size_t i = next.fetch_add(1);
                     if (i >= all.size()) break;
                     Planned& p = *all[i];
-                    p.cur = bam.fetch_begin(p.g.tid, p.g.start, p.g.end);
+                    Candidates& cur = p.cur.emplace(bam, p.g.tid, p.g.start, p.g.end, req_mapped);
                     const size_t want = p.g.n < 0 ? (size_t)-1 : (size_t)p.g.n * 2 + 32;
-                    // packed right after each fetch: record bytes live in the cursor's buffer until the next fetch_more
-                    while (!p.cur.done && p.pc.recs.size() < want) {
-                        recs.clear();
-                        bam.fetch_more(p.cur, std::min<size_t>(want - p.pc.recs.size(), 4096), [&](const RecRef& r) { return sampler_flag_ok(r, req_mapped); }, &recs);
-                        for (auto& r : recs) { pack_record(p.cur.bytes(r), r.size, &p.pc); p.pc.recs.push_back(r); }
-                    }
+                    while (!cur.done && p.pc.recs.size() < want) cur.more(std::min<size_t>(want - p.pc.recs.size(), 4096), &p.pc);
                 }
             } catch (...) { std::lock_guard<std::mutex> g(mu); if (!err) err = std::current_exception(); }
         };
@@ -599,119 +461,171 @@ inline size_t sample_histogram_indexed(const BamReader& bam, mkp_ctx* ctx, const
     for (auto& cp : cps) {
         if (bulks.empty() || cfg.include) { bulks.emplace_back(); bulks.back().tid = cp.tid; }
         cp.bulk = bulks.size() - 1;
-        Bulk& B = bulks.back();
-        for (auto& p : cp.plan) { p.lo = B.pc.recs.size(); append_packed(p.pc, &B.pc); p.hi = B.pc.recs.size(); p.pc.clear(); p.pc.heap.shrink_to_fit(); p.pc.hdrs.shrink_to_fit(); }
+        Bulk& bk = bulks.back();
+        for (auto& p : cp.plan) { p.lo = bk.pc.recs.size(); append_packed(p.pc, &bk.pc); p.hi = bk.pc.recs.size(); p.pc.clear(); p.pc.heap.shrink_to_fit(); p.pc.hdrs.shrink_to_fit(); }
     }
-    t_fetch += secs_between(tf0, clk::now());
+    res.fetch_s = std::chrono::duration<double>(clk::now() - tf0).count();
     trace_clock().mark(coll.rank, "sampler: candidates fetched + packed");
     if (cfg.device_ready) cfg.device_ready->wait();
     size_t resident_bulk = (size_t)-1;
-    for (size_t bi = 0; bi < bulks.size(); bi++) { bulks[bi].take.assign(bulks[bi].pc.recs.size(), 0); contributes_of(bulks[bi].pc, bulks[bi].tid, &bulks[bi].contributes); resident_bulk = bi; }
+    for (size_t bi = 0; bi < bulks.size(); bi++) { bulks[bi].take.assign(bulks[bi].pc.recs.size(), 0); decode(bulks[bi].pc, bulks[bi].tid, &bulks[bi].contributes); resident_bulk = bi; }
     trace_clock().mark(coll.rank, "sampler: candidates decoded on the device");
     size_t n_on_demand = 0;
     // ---- the real schedule, contig by contig
     for (auto& cp : cps) {
         const uint32_t t = cp.tid;
         std::vector<Planned>& plan = cp.plan;
-        Bulk& B = bulks[cp.bulk];
+        Bulk& bk = bulks[cp.bulk];
         std::map<std::string, size_t> by_key;
         for (size_t i = 0; i < plan.size(); i++) by_key.emplace(key_of(plan[i].g), i);
         std::unordered_set<uint64_t> selected;
         size_t done = 0;
         PackedChunk extra;
         std::vector<uint8_t> xcontrib, xtake;
-        std::vector<RecRef> recs;
         for (size_t s = 0; s < sbs.size(); s++) for (const Grp& g : todo_for(s, t, done)) {
             if (cfg.include && !cfg.include->overlaps_any(g.tid, g.start, g.end)) continue;
+            const size_t limit = g.n < 0 ? (size_t)-1 : (size_t)g.n;
             size_t used = 0;
-            BamReader::FetchCursor own;
-            BamReader::FetchCursor* curp = &own;
+            std::optional<Candidates> own;
+            Candidates* cur;
             auto it = by_key.find(key_of(g));
             if (it != by_key.end() && !plan[it->second].used) {
                 Planned& p = plan[it->second];
                 p.used = true;
-                for (size_t k = p.lo; k < p.hi && (g.n < 0 || used < (size_t)g.n); k++) {
-                    if (!B.contributes[k]) continue;
-                    used++;
-                    if (selected.insert(B.pc.recs[k].off).second) B.take[k] = 1;
-                }
-                curp = &p.cur;             // (stays with the plan: its buffers are released with the rest, see defer_free)
-            } else own = bam.fetch_begin(g.tid, g.start, g.end);
-            BamReader::FetchCursor& cur = *curp;
+                select_first(bk.pc.recs, bk.contributes, p.lo, p.hi, limit, &used, &selected, &bk.take);
+                cur = &*p.cur;             // (stays with the plan: its buffers are released with the rest, see defer_free)
+            } else cur = &own.emplace(bam, g.tid, g.start, g.end, req_mapped);
             // on demand: the plan did not cover the group, or the group needs more candidates than were fetched
-            while (!cur.done && (g.n < 0 || used < (size_t)g.n)) {
+            while (!cur->done && used < limit) {
                 n_on_demand++;
-                const size_t want = g.n < 0 ? 4096 : ((size_t)g.n - used) * 2 + 32;
                 extra.clear();
-                recs.clear();
-                bam.fetch_more(cur, want, [&](const RecRef& r) { return sampler_flag_ok(r, req_mapped); }, &recs);
-                for (auto& r : recs) { pack_record(cur.bytes(r), r.size, &extra); extra.recs.push_back(r); }
+                cur->more(g.n < 0 ? 4096 : (limit - used) * 2 + 32, &extra);
                 if (extra.recs.empty()) continue;
-                contributes_of(extra, t, &xcontrib);
+                decode(extra, t, &xcontrib);
                 resident_bulk = (size_t)-1;
                 xtake.assign(extra.recs.size(), 0);
-                for (size_t k = 0; k < extra.recs.size() && (g.n < 0 || used < (size_t)g.n); k++) {
-                    if (!xcontrib[k]) continue;
-                    used++;
-                    if (selected.insert(extra.recs[k].off).second) xtake[k] = 1;
-                }
+                select_first(extra.recs, xcontrib, 0, extra.recs.size(), limit, &used, &selected, &xtake);
                 add_taken(xtake);
-                if (keep) { bool any = false; for (uint8_t x : xtake) any = any || x; if (any) keep->push_back({extra, xtake, t}); }
+                keep(PackedChunk(extra), std::vector<uint8_t>(xtake), t);
             }
             done += used;
         }
-        n_selected += selected.size();
+        res.n_selected += selected.size();
     }
     if (trace_clock().on) fprintf(stderr, "[mkh r%d]             sampler: %zu on-demand fetches during the replay\n", coll.rank, n_on_demand);
     trace_clock().mark(coll.rank, "sampler: schedule replayed");
     // ---- histogram of the selected reads of every bulk chunk
     for (size_t bi = 0; bi < bulks.size(); bi++) {
-        Bulk& B = bulks[bi];
-        bool any = false;
-        for (uint8_t x : B.take) any = any || x;
-        if (!any) continue;
-        if (resident_bulk != bi) { upload(B.pc, B.tid); resident_bulk = bi; }
-        add_taken(B.take);
-        if (keep) keep->push_back({std::move(B.pc), std::move(B.take), B.tid});
+        Bulk& bk = bulks[bi];
+        if (!any(bk.take)) continue;
+        if (resident_bulk != bi) { upload_sampled(bam, ctx, bk.pc, bk.tid, cfg.include); resident_bulk = bi; }
+        add_taken(bk.take);
+        keep(std::move(bk.pc), std::move(bk.take), bk.tid);
     }
     trace_clock().mark(coll.rank, "sampler: histogram of the selection");
-    if (!only_mapped) {   // reads without coordinates (reads_sampler/mod.rs:85-129): the last rank, after the global count is known
-        uint64_t cnt[1] = {n_selected};
+    if (cfg.include_unmapped) {   // reads without coordinates (reads_sampler/mod.rs:85-129): the last rank, after the global count is known
+        uint64_t cnt[1] = {res.n_selected};
         coll.sum(cnt, 1);
         if (coll.rank == coll.world - 1) {
             const size_t limit = cfg.take_all ? (size_t)-1 : (cfg.num_reads > cnt[0] ? cfg.num_reads - (size_t)cnt[0] : 0);
             PackedChunk cand;
-            BamReader::FetchCursor cur = bam.fetch_unplaced_begin();
-            std::vector<RecRef> recs;
-            while (!cur.done) {
-                recs.clear();
-                bam.fetch_more(cur, 4096, [&](const RecRef& r) { return sampler_flag_ok(r, cfg.edge_on); }, &recs);
-                for (auto& r : recs) { pack_record(cur.bytes(r), r.size, &cand); cand.recs.push_back(r); }
-            }
+            Candidates cur(bam, -1, 0, 0, cfg.edge_on);
+            while (!cur.done) cur.more(4096, &cand);
             if (!cand.recs.empty()) {
                 std::vector<uint8_t> contributes, take(cand.recs.size(), 0);
-                contributes_of(cand, 0, &contributes);
+                decode(cand, 0, &contributes);
                 size_t used = 0;
-                for (size_t k = 0; k < cand.recs.size() && used < limit; k++) { if (!contributes[k]) continue; used++; take[k] = 1; }
+                std::unordered_set<uint64_t> none;
+                select_first(cand.recs, contributes, 0, cand.recs.size(), limit, &used, &none, &take);
                 add_taken(take);
-                n_selected += used;
-                if (keep && used) keep->push_back({std::move(cand), std::move(take), 0});
+                res.n_selected += used;
+                keep(std::move(cand), std::move(take), 0);
             }
         }
     }
     // ---- the one exchange of a sharded run: sum of the histograms (+ the inexact-value count and the read count)
     if (coll.world > 1) {
-        std::vector<uint64_t> buf(4 * MKP_HIST_BINS + 2);
-        memcpy(buf.data(), hist, 4 * MKP_HIST_BINS * sizeof(uint64_t));
-        buf[4 * MKP_HIST_BINS] = inexact_local; buf[4 * MKP_HIST_BINS + 1] = n_selected;
+        std::vector<uint64_t> buf(res.hist);
+        buf.push_back(res.inexact);
+        buf.push_back(res.n_selected);
         coll.sum(buf.data(), buf.size());
-        memcpy(hist, buf.data(), 4 * MKP_HIST_BINS * sizeof(uint64_t));
-        inexact_local = buf[4 * MKP_HIST_BINS]; n_selected = buf[4 * MKP_HIST_BINS + 1];
+        std::copy(buf.begin(), buf.begin() + 4 * MKP_HIST_BINS, res.hist.begin());
+        res.inexact = buf[4 * MKP_HIST_BINS]; res.n_selected = buf[4 * MKP_HIST_BINS + 1];
     }
-    if (inexact) *inexact = inexact_local;
-    if (fetch_s) *fetch_s = t_fetch;
     if (cfg.defer_free) *cfg.defer_free = heavy;
-    return (size_t)n_selected;
+    return res;
+}
+
+// --sampling-frac / --no-sampling and the schedule's other options. Only -f 1.0 is reproducible without the reference's RNG;
+// `alternatives` names the command's other ways to choose the reads.
+inline SamplerConfig sampler_config(int threads, uint32_t sampling_interval_size, size_t num_reads, bool have_frac, double frac, bool no_sampling, const char* alternatives) {
+    if (!no_sampling && have_frac && frac != 1.0) throw std::runtime_error(std::string("only --sampling-frac 1.0 is reproducible without the reference's RNG; use ") + alternatives);
+    SamplerConfig sc;
+    sc.threads = sc.workers = threads;
+    sc.sampling_interval_size = sampling_interval_size;
+    sc.take_all = no_sampling || have_frac;
+    sc.num_reads = num_reads;
+    return sc;
+}
+
+// a quantile of the histogram is exact only when every sampled value lies on its 1/1024 grid; `hint` ends the error otherwise
+inline void require_exact(uint64_t inexact, const char* hint) {
+    if (inexact) throw std::runtime_error("sampled probabilities are not multiples of 1/1024 (" + std::to_string(inexact) + " values): " + hint);
+}
+
+// The estimated thresholds (command_utils.rs:74-134, thresholds.rs:118-156): the `percentile` quantile of every base the sample
+// has values for. `announce`: print pileup's "> Using filter threshold" lines.
+inline void estimated_thresholds(const SampleResult& s, float percentile, const char* inexact_hint, bool announce, mkp_params* P) {
+    require_exact(s.inexact, inexact_hint);
+    for (int b = 0; b < 4; b++) {
+        const uint64_t* h = s.hist.data() + b * MKP_HIST_BINS;
+        if (std::all_of(h, h + MKP_HIST_BINS, [](uint64_t v) { return v == 0; })) continue;
+        float thr;
+        if (!percentile_from_hist(h, percentile, &thr)) throw std::runtime_error("not enough datapoints to estimate a threshold");
+        P->base_threshold_set[b] = 1;
+        P->base_threshold[b] = thr;
+        if (announce) fprintf(stderr, "> Using filter threshold %.9g for %c.\n", thr, "ACGT"[b]);
+    }
+}
+
+// ---- the filter flags shared by pileup, pileup-hemi, summary and sample-probs (command_utils.rs:18-73, 243-275)
+// --edge-filter N | START,END and --invert-edge-filter
+inline void parse_edge_filter(const std::string& raw, bool invert, mkp_params* P) {
+    if (raw.empty()) return;
+    P->edge_filter_on = 1; P->edge_filter_inverted = invert;
+    auto c = raw.find(',');
+    if (c == std::string::npos) P->edge_filter_start = P->edge_filter_end = (uint32_t)std::stoul(raw);
+    else { P->edge_filter_start = (uint32_t)std::stoul(raw.substr(0, c)); P->edge_filter_end = (uint32_t)std::stoul(raw.substr(c + 1)); }
+}
+// --mod-thresholds CODE:VALUE (repeatable)
+inline void parse_mod_thresholds(const std::vector<std::string>& raws, mkp_params* P) {
+    for (auto& raw : raws) {
+        auto c = raw.find(':');
+        uint32_t code;
+        if (c == std::string::npos || raw.find(':', c + 1) != std::string::npos || !parse_code(raw.substr(0, c), &code))
+            throw std::runtime_error("encountered illegal per-mod threshold: " + raw + ". Should be mod_code:threshold e.g. h:0.8");
+        if (P->n_mod_thresholds >= MKP_MAX_MOD_THRESHOLDS) throw std::runtime_error("too many per-mod thresholds");
+        P->mod_code[P->n_mod_thresholds] = code;
+        P->mod_threshold[P->n_mod_thresholds++] = std::stof(raw.substr(c + 1));
+    }
+}
+// --filter-threshold [BASE:]VALUE (repeatable): one default, one per base
+inline void parse_filter_thresholds(const std::vector<std::string>& raws, mkp_params* P) {
+    bool have_default = false;
+    for (auto& raw : raws) {
+        auto c = raw.find(':');
+        if (c == std::string::npos) {
+            if (have_default) throw std::runtime_error("default threshold encountered more than once");
+            P->default_threshold = std::stof(raw); have_default = true;
+        } else {
+            const char* B = "ACGT";
+            const char* f = raw.empty() ? nullptr : strchr(B, raw[0]);
+            if (!f || !raw[0]) throw std::runtime_error("failed to parse base " + raw);
+            if (P->base_threshold_set[f - B]) throw std::runtime_error(std::string("repeated threshold for base ") + raw[0]);
+            P->base_threshold_set[f - B] = 1;
+            P->base_threshold[f - B] = std::stof(raw.substr(c + 1));
+        }
+    }
 }
 
 // htslib bam_plp_push with maxcnt (sam.c): the engine drops the reads of its flag mask first (they never count), keeps the
@@ -833,12 +747,7 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
         if (o.traditional) { P.numeric_mode = 2; P.collapse_code = 'h'; combine_strands = true; }
         else if (o.combine_mods) P.numeric_mode = 1;
         else if (!o.ignore.empty()) { uint32_t c; if (!parse_code(o.ignore, &c)) throw std::runtime_error("failed to parse mod code " + o.ignore); P.numeric_mode = 2; P.collapse_code = c; }
-        if (!o.edge.empty()) {
-            P.edge_filter_on = 1; P.edge_filter_inverted = o.invert_edge;
-            auto c = o.edge.find(',');
-            if (c == std::string::npos) P.edge_filter_start = P.edge_filter_end = (uint32_t)std::stoul(o.edge);
-            else { P.edge_filter_start = (uint32_t)std::stoul(o.edge.substr(0, c)); P.edge_filter_end = (uint32_t)std::stoul(o.edge.substr(c + 1)); }
-        }
+        parse_edge_filter(o.edge, o.invert_edge, &P);
         // motifs (subcommand.rs:526-539, 592-612)
         std::vector<std::string> parts = o.motif_parts;
         MotifContext mc;
@@ -875,43 +784,41 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
         std::vector<RefInterval> ivs = interval_grid(iv_targets, o.interval_size, combine_strands, have_motifs ? &mc : nullptr, &iv_owner);
         size_t my_i0 = 0, my_i1 = ivs.size();
         if (sharded) { const std::vector<size_t> cuts = shard_cuts(bam, ivs, coll.world); my_i0 = cuts[coll.rank]; my_i1 = cuts[coll.rank + 1]; }
-        // ---- threshold estimation starts now when it can run beside the load: its candidates come straight from the file (host
-        // fetch through the index), only its decode passes need the device and wait for `dev_ready`
+        // ---- threshold estimation. With the device ingest of an indexed BAM it starts now, beside the load: its candidates come
+        // straight from the file (host fetch through the index), only its decode passes need the device and wait for `dev_ready`.
+        // Otherwise it runs after the load, on the reads of the pileup.
         const bool estimate = o.filter_thresholds.empty() && !o.no_filtering;
-        std::vector<uint64_t> bg_hist(4 * MKP_HIST_BINS);
-        uint64_t bg_inexact = 0;
-        double bg_fetch_s = 0;
-        std::exception_ptr bg_err;
-        std::promise<void> dev_ready_p;
+        SamplerConfig sc;
+        SampleResult sample;
+        std::exception_ptr sample_err;
+        std::shared_ptr<void> sample_garbage;
+        std::promise<void> dev_ready_p, sample_done_p;
         std::shared_future<void> dev_ready_f = dev_ready_p.get_future().share();
+        std::future<void> sample_done_f = sample_done_p.get_future();
         bool dev_ready_set = false;
-        SamplerConfig bg_sc;
-        std::shared_ptr<void> bg_garbage;
-        std::promise<void> bg_result_p;
-        std::future<void> bg_result_f = bg_result_p.get_future();
+        auto run_sampler = [&](const BamReader& src) {
+            try { sample = sample_histogram(src, dev.ctx, sc, coll); }
+            catch (...) { sample_err = std::current_exception(); }
+            sample_done_p.set_value();           // the result is out; the candidate buffers are released after that, beside the pileup
+            sample_garbage.reset();
+        };
         struct BgJoin { std::thread t; std::promise<void>* p; bool* set; ~BgJoin() { if (!*set) { try { p->set_value(); } catch (...) {} *set = true; } if (t.joinable()) t.join(); } } bg_job{std::thread(), &dev_ready_p, &dev_ready_set};
         trace("interval grid + shard cuts");
-        const bool sampler_bg = estimate && !loaded && bam.have_index();
-        if (sampler_bg) {
-            if (o.have_frac && o.frac != 1.0) throw std::runtime_error("only --sampling-frac 1.0 is reproducible without the reference's RNG; use -n or -f 1.0");
+        if (estimate) {
+            sc = sampler_config(o.schedule_threads > 0 ? o.schedule_threads : o.threads, o.sampling_interval_size, o.num_reads, o.have_frac, o.frac, false, "-n or -f 1.0");
+            sc.workers = o.threads;
+            sc.region = srp ? srp : rp;
+            sc.include_unmapped = o.include_unmapped;
+            sc.edge_on = P.edge_filter_on;
+            sc.include = inc;
+            sc.defer_free = &sample_garbage;
             mkp_params PS = P;
             PS.max_depth = 0;           // the sampler looks at reads, not at pileup columns
             if (mkp_set_params(dev.ctx, &PS)) throw std::runtime_error(mkp_last_error(dev.ctx));
-            bg_sc.threads = o.schedule_threads > 0 ? o.schedule_threads : o.threads; bg_sc.workers = o.threads; bg_sc.sampling_interval_size = o.sampling_interval_size;
-            bg_sc.take_all = o.have_frac;
-            bg_sc.num_reads = o.num_reads;
-            bg_sc.region = srp ? srp : rp;
-            bg_sc.include_unmapped = o.include_unmapped;
-            bg_sc.edge_on = P.edge_filter_on;
-            bg_sc.include = inc;
-            bg_sc.device_ready = &dev_ready_f;
-            bg_sc.defer_free = &bg_garbage;
-            bg_job.t = std::thread([&]() {
-                try { sample_histogram_indexed(bam, dev.ctx, bg_sc, bg_hist.data(), &bg_inexact, coll, &bg_fetch_s); }
-                catch (...) { bg_err = std::current_exception(); }
-                bg_result_p.set_value();           // the result is out; the candidate buffers are released after that, beside the pileup
-                bg_garbage.reset();
-            });
+            if (!loaded && bam.have_index()) {
+                sc.device_ready = &dev_ready_f;
+                bg_job.t = std::thread(run_sampler, std::cref(bam));
+            }
         }
         // ---- focus positions of this rank's intervals (reference motif scan), beside the load and the sampler. Every object the
         // job touches is declared above; its joiner is declared after them, so it is destroyed (joined) before they are.
@@ -926,6 +833,7 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
             } catch (...) { iv_err = std::current_exception(); }
         });
         // ---- device load: everything, or the byte ranges under this rank's intervals
+        std::optional<BamReader> host_bam;
         if (!loaded) {
             if (sharded) {
                 std::vector<BamReader::Piece> pieces;
@@ -937,19 +845,21 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
             } else {
                 try { bam.load_default(); }
                 catch (const DeviceIngestTooBig& e) {
-                    // a front-end choice, not a compute fallback: the reads are sliced on the host and uploaded chunk by chunk
+                    // a front-end choice, not a compute fallback: the reads are sliced on the host and uploaded chunk by chunk. A
+                    // reader of its own: the sampler may still be fetching through `bam`.
                     if (!o.quiet) fprintf(stderr, "> %s; reading the BAM on the host instead\n", e.what());
-                    bam = BamReader();
-                    bam.open(o.in_bam, o.threads);
+                    host_bam.emplace();
+                    host_bam->open(o.in_bam, o.threads);
                 }
             }
         }
+        BamReader& reads = host_bam ? *host_bam : bam;       // the records of the pileup
         if (!dev_ready_set) { dev_ready_p.set_value(); dev_ready_set = true; }
         const auto t_load = clk::now();
         trace("device load done");
-        if (trace_clock().on) fprintf(stderr, "[mkh r%d]             ingest: h2d %.1f ms, inflate %.1f ms, record walk %.1f ms, total %.1f ms\n", coll.rank, bam.ingest_ms[0], bam.ingest_ms[1], bam.ingest_ms[2], bam.ingest_ms[3]);
+        if (trace_clock().on) fprintf(stderr, "[mkh r%d]             ingest: h2d %.1f ms, inflate %.1f ms, record walk %.1f ms, total %.1f ms\n", coll.rank, reads.ingest_ms[0], reads.ingest_ms[1], reads.ingest_ms[2], reads.ingest_ms[3]);
         uint64_t any_mapped = 0;
-        for (auto& t : targets) if (rp || !inc || inc->has_contig(t.tid)) any_mapped += bam.stats.n_mapped[t.tid];
+        for (auto& t : targets) if (rp || !inc || inc->has_contig(t.tid)) any_mapped += reads.stats.n_mapped[t.tid];
         if (!any_mapped) throw std::runtime_error("did not find any mapped reads, perform alignment first or use modkit extract and/or modkit summary to inspect unaligned modBAMs");
         // output first, like the reference, so a bad path fails before any work
         FILE* out = nullptr;
@@ -996,78 +906,14 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
         const std::string pfx = o.prefix.empty() ? std::string() : o.prefix + "_";
 
         // thresholds (subcommand.rs:615-638, command_utils.rs:49-134)
-        for (auto& raw : o.mod_thresholds) {
-            auto c = raw.find(':');
-            uint32_t code;
-            if (c == std::string::npos || raw.find(':', c + 1) != std::string::npos || !parse_code(raw.substr(0, c), &code))
-                throw std::runtime_error("encountered illegal per-mod threshold: " + raw + ". Should be mod_code:threshold e.g. h:0.8");
-            if (P.n_mod_thresholds >= MKP_MAX_MOD_THRESHOLDS) throw std::runtime_error("too many per-mod thresholds");
-            P.mod_code[P.n_mod_thresholds] = code;
-            P.mod_threshold[P.n_mod_thresholds++] = std::stof(raw.substr(c + 1));
-        }
-        double fetch_s = 0;
-        if (!o.filter_thresholds.empty()) {
-            bool have_default = false;
-            for (auto& raw : o.filter_thresholds) {
-                auto c = raw.find(':');
-                if (c == std::string::npos) {
-                    if (have_default) throw std::runtime_error("default threshold encountered more than once");
-                    P.default_threshold = std::stof(raw); have_default = true;
-                } else {
-                    const char* B = "ACGT";
-                    const char* f = raw.empty() ? nullptr : strchr(B, raw[0]);
-                    if (!f || !raw[0]) throw std::runtime_error("failed to parse base " + raw);
-                    if (P.base_threshold_set[f - B]) throw std::runtime_error(std::string("repeated threshold for base ") + raw[0]);
-                    P.base_threshold_set[f - B] = 1;
-                    P.base_threshold[f - B] = std::stof(raw.substr(c + 1));
-                }
-            }
-        } else if (!o.no_filtering && sampler_bg) {
-            bg_result_f.wait();
+        parse_mod_thresholds(o.mod_thresholds, &P);
+        parse_filter_thresholds(o.filter_thresholds, &P);
+        if (estimate) {
+            if (!bg_job.t.joinable()) run_sampler(reads);
+            sample_done_f.wait();
             trace("sampler result");
-            if (bg_err) std::rethrow_exception(bg_err);
-            fetch_s = bg_fetch_s;
-            if (bg_inexact) throw std::runtime_error("sampled probabilities are not multiples of 1/1024 (" + std::to_string(bg_inexact) + " values): exact histogram quantile impossible; pass --filter-threshold");
-            for (int b = 0; b < 4; b++) {
-                float thr;
-                uint64_t n = 0;
-                for (int k = 0; k < MKP_HIST_BINS; k++) n += bg_hist[b * MKP_HIST_BINS + k];
-                if (!n) continue;
-                if (!percentile_from_hist(bg_hist.data() + b * MKP_HIST_BINS, o.percentile, &thr)) throw std::runtime_error("not enough datapoints to estimate a threshold");
-                P.base_threshold_set[b] = 1;
-                P.base_threshold[b] = thr;
-                if (!o.quiet && coll.rank == 0) fprintf(stderr, "> Using filter threshold %.9g for %c.\n", thr, "ACGT"[b]);
-            }
-        } else if (!o.no_filtering) {
-            mkp_params PS = P;
-            PS.max_depth = 0;           // the sampler looks at reads, not at pileup columns
-            if (mkp_set_params(dev.ctx, &PS)) throw std::runtime_error(mkp_last_error(dev.ctx));
-            SamplerConfig sc;
-            sc.threads = o.schedule_threads > 0 ? o.schedule_threads : o.threads; sc.workers = o.threads; sc.sampling_interval_size = o.sampling_interval_size;
-            if (o.have_frac) { if (o.frac != 1.0) throw std::runtime_error("only --sampling-frac 1.0 is reproducible without the reference's RNG; use -n or -f 1.0"); sc.take_all = true; }
-            sc.num_reads = o.num_reads;
-            sc.region = srp ? srp : rp;
-            sc.include_unmapped = o.include_unmapped;
-            sc.edge_on = P.edge_filter_on;
-            sc.include = inc;
-            std::vector<uint64_t> hist(4 * MKP_HIST_BINS);
-            uint64_t inexact = 0;
-            if (bam.on_device && bam.have_index()) sample_histogram_indexed(bam, dev.ctx, sc, hist.data(), &inexact, coll, &fetch_s);
-            else {
-                if (sharded) throw std::runtime_error("interval-sharded runs need a BAM index (.bai)");
-                sample_histogram(bam, dev.ctx, sc, hist.data(), &inexact);
-            }
-            if (inexact) throw std::runtime_error("sampled probabilities are not multiples of 1/1024 (" + std::to_string(inexact) + " values): exact histogram quantile impossible; pass --filter-threshold");
-            for (int b = 0; b < 4; b++) {
-                float thr;
-                uint64_t n = 0;
-                for (int k = 0; k < MKP_HIST_BINS; k++) n += hist[b * MKP_HIST_BINS + k];
-                if (!n) continue;
-                if (!percentile_from_hist(hist.data() + b * MKP_HIST_BINS, o.percentile, &thr)) throw std::runtime_error("not enough datapoints to estimate a threshold");
-                P.base_threshold_set[b] = 1;
-                P.base_threshold[b] = thr;
-                if (!o.quiet && coll.rank == 0) fprintf(stderr, "> Using filter threshold %.9g for %c.\n", thr, "ACGT"[b]);
-            }
+            if (sample_err) std::rethrow_exception(sample_err);
+            estimated_thresholds(sample, o.percentile, "exact histogram quantile impossible; pass --filter-threshold", !o.quiet && coll.rank == 0, &P);
         }
         if (mkp_set_params(dev.ctx, &P)) throw std::runtime_error(mkp_last_error(dev.ctx));
         if (summary) for (int b = 0; b < 4; b++) { summary->thresholds[b] = P.base_threshold[b]; summary->threshold_set[b] = P.base_threshold_set[b]; }
@@ -1079,7 +925,7 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
         const auto t_iv = clk::now();
         (void)t_iv;
         RunSummary S;
-        S.fetch_s = fetch_s;
+        S.fetch_s = sample.fetch_s;
         if (sharded) { ivs.erase(ivs.begin() + (ptrdiff_t)my_i1, ivs.end()); ivs.erase(ivs.begin(), ivs.begin() + (ptrdiff_t)my_i0); }
         for (auto& iv : ivs) S.positions += iv.end - iv.start;
 
@@ -1111,8 +957,8 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
                     if (ivs[c1 - 1].end <= ivs[c0].start) { c0 = c1; continue; }
                     // the reads of the chunk
                     std::vector<RecRef> chunk_recs;
-                    bam.ensure_tid(ivs[c0].tid);
-                    bam.for_overlapping(ivs[c0].tid, ivs[c0].start, ivs[c1 - 1].end, [&](const RecRef& r) { chunk_recs.push_back(r); });
+                    reads.ensure_tid(ivs[c0].tid);
+                    reads.for_overlapping(ivs[c0].tid, ivs[c0].start, ivs[c1 - 1].end, [&](const RecRef& r) { chunk_recs.push_back(r); });
                     if (chunk_recs.empty()) { c0 = c1; continue; }
                     // --max-depth (src/pileup/mod.rs:755-759 -> bam_plp_set_maxcnt): the pileup engine of the reference runs per interval
                     // and drops reads while its buffer is full, so the reads that count can differ from interval to interval. Only a
@@ -1141,7 +987,7 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
                         // pileup-hemi: the call window reaches the partner of every motif position; the reads stay those of the intervals
                         uint32_t wcs = cs, wce = ce;
                         if (hemi_partner < 0) wcs = cs - std::min<uint32_t>(cs, (uint32_t)-hemi_partner);
-                        if (hemi_partner > 0) wce = (uint32_t)std::min<uint64_t>((uint64_t)ce + (uint32_t)hemi_partner, std::max(ce, bam.ref_lens[ivs[i0].tid]));
+                        if (hemi_partner > 0) wce = (uint32_t)std::min<uint64_t>((uint64_t)ce + (uint32_t)hemi_partner, std::max(ce, reads.ref_lens[ivs[i0].tid]));
                         std::vector<RecRef>& all_recs = wk.recs;
                         // with --partition-tag one group per key (each an independent pileup: src/pileup/mod.rs:795-830), in key order
                         std::map<std::string, std::vector<RecRef>> groups;
@@ -1152,7 +998,7 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
                             for (auto& r : all_recs) if (!((r.flag & (0x4 | 0x100 | 0x200 | 0x400 | 0x800)) || r.l_seq == 0)) adm.push_back(r);
                             std::vector<uint8_t> cells;
                             const size_t n_pt = o.partition_tags.size();
-                            if (bam.on_device && !adm.empty()) {
+                            if (reads.on_device && !adm.empty()) {
                                 std::vector<uint32_t> ids(adm.size());
                                 for (size_t k = 0; k < adm.size(); k++) ids[k] = adm[k].idx;
                                 cells.resize(adm.size() * n_pt * MKP_TAG_CELL);
@@ -1170,8 +1016,8 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
                             }
                             for (size_t k = 0; k < adm.size(); k++) {
                                 std::string key;
-                                const bool have = bam.on_device ? partition_key_of_cells(cells.data() + k * n_pt * MKP_TAG_CELL, n_pt, &key)
-                                                                : partition_key_of(bam.rec(adm[k]), adm[k].size, o.partition_tags, &key);
+                                const bool have = reads.on_device ? partition_key_of_cells(cells.data() + k * n_pt * MKP_TAG_CELL, n_pt, &key)
+                                                                  : partition_key_of(reads.rec(adm[k]), adm[k].size, o.partition_tags, &key);
                                 groups[have ? key : std::string("\1")].push_back(adm[k]);
                             }
                         }
@@ -1179,8 +1025,8 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
                         for (auto& grp : groups) {
                             const auto ta = clk::now();
                             pc.clear();
-                            if (bam.on_device) pc.recs = grp.second;
-                            else pack_records_mt(bam, grp.second, o.threads, &pc);
+                            if (reads.on_device) pc.recs = grp.second;
+                            else pack_records_mt(reads, grp.second, o.threads, &pc);
                             if (pc.recs.empty()) continue;
                             mkp_chunk ch;
                             memset(&ch, 0, sizeof ch);
@@ -1197,9 +1043,9 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
                                 for (size_t k = i0; k < i1; k++) starts.push_back(ivs[k].start);
                                 if (mkp_hemi_resident(dev.ctx, starts.data(), (uint32_t)starts.size(), hemi_partner, &st)) throw std::runtime_error(mkp_last_error(dev.ctx));
                             };
-                            if (bam.on_device) {
+                            if (reads.on_device) {
                                 // slice on the GPU (no packed chunk in host memory), then the same kernels
-                                device_chunk(bam, pc.recs, wcs, wce, ch.focus_pos, ch.focus_neg);
+                                device_chunk(reads, pc.recs, wcs, wce, ch.focus_pos, ch.focus_neg);
                                 const auto t_s = clk::now();
                                 S.slice_s += secs(tb, t_s);
                                 if (o.hemi) hemi_pass();
@@ -1227,7 +1073,7 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
                             S.gpu_s += secs(tb, clk::now());
                             S.kernel_ms += st.kernel_ms[7];
                             S.reads_packed += pc.recs.size();
-                            S.algorithmic_bytes += (want_alg_bytes || !bam.on_device ? pc.algorithmic_bytes() : 0) + (o.hemi ? sizeof(mkp_hemi_row) : sizeof(mkp_row)) * n_rows;
+                            S.algorithmic_bytes += (want_alg_bytes || !reads.on_device ? pc.algorithmic_bytes() : 0) + (o.hemi ? sizeof(mkp_hemi_row) : sizeof(mkp_row)) * n_rows;
                             S.chunks++;
                             push_out(std::move(co));
                         }
@@ -1262,7 +1108,7 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
             auto pos_of = [&](size_t j) { return o.hemi ? co.hemi_rows[j].pos : rows[j].pos; };
             const std::string& key_name = co.key_name;
             // rows are position sorted: every interval gets its slice; intervals are finished and formatted in parallel
-            const std::string& chrom = bam.ref_names[ivs[i0].tid];
+            const std::string& chrom = reads.ref_names[ivs[i0].tid];
             const size_t n_iv = i1 - i0;
             std::vector<size_t> rlo(n_iv + 1);
             {
@@ -1397,7 +1243,7 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
                 fprintf(jf, "{\"positions\": %llu, \"rows\": %llu, \"reads\": %llu, \"chunks\": %llu, \"algorithmic_bytes\": %llu, \"load_s\": %.6f, \"thresholds_s\": %.6f, \"intervals_s\": %.6f, \"pack_s\": %.6f, \"gpu_s\": %.6f, \"kernel_ms\": %.6f, \"write_s\": %.6f, \"total_s\": %.6f, \"ingest\": \"%s\", \"ingest_h2d_ms\": %.3f, \"ingest_inflate_ms\": %.3f, \"ingest_walk_ms\": %.3f, \"sampler_fetch_s\": %.6f, \"slice_s\": %.6f, \"pass_s\": %.6f, \"rowcopy_s\": %.6f}\n",
                         (unsigned long long)S.positions, (unsigned long long)S.rows, (unsigned long long)S.reads_packed, (unsigned long long)S.chunks, (unsigned long long)S.algorithmic_bytes,
                         S.load_s, S.threshold_s, S.interval_s, S.pack_s, S.gpu_s, S.kernel_ms, S.write_s, S.total_s,
-                        bam.on_device ? (bam.ranged() ? "device-ranged" : "device") : "host", bam.ingest_ms[0], bam.ingest_ms[1], bam.ingest_ms[2], S.fetch_s, S.slice_s, S.pass_s, S.rowcopy_s);
+                        reads.on_device ? (reads.ranged() ? "device-ranged" : "device") : "host", reads.ingest_ms[0], reads.ingest_ms[1], reads.ingest_ms[2], S.fetch_s, S.slice_s, S.pass_s, S.rowcopy_s);
                 fclose(jf);
             }
         }
@@ -1405,7 +1251,7 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
             trace("stats written");
             std::vector<RefInterval>().swap(ivs); trace("intervals released");
             part_pool.clear(); part_pool.shrink_to_fit(); shard_parts.clear(); shard_parts.shrink_to_fit(); spare_rows.clear(); spare_rows.shrink_to_fit(); trace("text + row buffers released");
-            bam.release_host_tables(); trace("record tables released");
+            reads.release_host_tables(); trace("record tables released");
         }
         return 0;
     } catch (const std::exception& e) {
@@ -1575,12 +1421,11 @@ inline std::string f64_display(double v) {
     return std::string(buf, r.ptr);
 }
 
-// sampling + thresholds shared by both commands; fills the kept chunks when `keep` is given. `inexact` receives the count of
-// sampled values off the histogram's 1/1024 grid: only a quantile of the histogram needs them on it
-inline void sample_for_summary(const SampleOptions& o, mkp_ctx* ctx, BamReader& bam, mkp_params* P, Region* region_out, bool* have_region, IncludeBed* include, bool* have_include,
-                               std::vector<uint64_t>* hist, std::vector<SampledChunk>* keep, size_t* n_selected, uint64_t* inexact_out) {
-    try { bam.open_device_index(o.in_bam, ctx); }
-    catch (...) { throw; }
+// the sampled reads of both commands: the reader (a file without index is read on the host), the filters, the schedule.
+// `keep`: also return the sampled reads themselves
+inline SampleResult sample_for_summary(const SampleOptions& o, mkp_ctx* ctx, bool keep, BamReader& bam, mkp_params* P, Region* region_out, bool* have_region,
+                                       IncludeBed* include, bool* have_include) {
+    bam.open_device_index(o.in_bam, ctx);
     if (!bam.have_index()) { bam = BamReader(); bam.open(o.in_bam, o.threads); }       // no index: the (small) file is read on the host
     *have_region = false;
     if (!o.region.empty()) { *region_out = parse_region_arg(o.region, bam); *have_region = true; }
@@ -1593,33 +1438,16 @@ inline void sample_for_summary(const SampleOptions& o, mkp_ctx* ctx, BamReader& 
     }
     memset(P, 0, sizeof *P);
     if (!o.ignore.empty()) { uint32_t c; if (!parse_code(o.ignore, &c)) throw std::runtime_error("failed to parse mod code " + o.ignore); P->numeric_mode = 2; P->collapse_code = c; }
-    if (!o.edge.empty()) {
-        P->edge_filter_on = 1; P->edge_filter_inverted = o.invert_edge;
-        auto c = o.edge.find(',');
-        if (c == std::string::npos) P->edge_filter_start = P->edge_filter_end = (uint32_t)std::stoul(o.edge);
-        else { P->edge_filter_start = (uint32_t)std::stoul(o.edge.substr(0, c)); P->edge_filter_end = (uint32_t)std::stoul(o.edge.substr(c + 1)); }
-    }
+    parse_edge_filter(o.edge, o.invert_edge, P);
     P->force_allow_implicit = 1;     // the sampler takes implicit lists as they are (no InvalidImplicitMode check outside the pileup)
     if (mkp_set_params(ctx, P)) throw std::runtime_error(mkp_last_error(ctx));
-    SamplerConfig sc;
-    sc.threads = o.threads; sc.workers = o.threads; sc.sampling_interval_size = o.interval_size;
-    if (o.no_sampling) sc.take_all = true;
-    else if (o.have_frac) { if (o.frac != 1.0) throw std::runtime_error("only --sampling-frac 1.0 is reproducible without the reference's RNG; use -n, -f 1.0 or --no-sampling"); sc.take_all = true; }
-    sc.num_reads = o.num_reads;
+    SamplerConfig sc = sampler_config(o.threads, o.interval_size, o.num_reads, o.have_frac, o.frac, o.no_sampling, "-n, -f 1.0 or --no-sampling");
     sc.region = *have_region ? region_out : nullptr;
     sc.include_unmapped = !(o.only_mapped || *have_include);
     sc.edge_on = P->edge_filter_on;
     sc.include = *have_include ? include : nullptr;
-    hist->assign(4 * MKP_HIST_BINS, 0);
-    uint64_t inexact = 0;
-    Collective solo;
-    if (bam.on_device && bam.have_index()) *n_selected = sample_histogram_indexed(bam, ctx, sc, hist->data(), &inexact, solo, nullptr, keep);
-    else *n_selected = sample_histogram(bam, ctx, sc, hist->data(), &inexact, keep);
-    *inexact_out = inexact;
-}
-
-inline void require_exact(uint64_t inexact) {
-    if (inexact) throw std::runtime_error("sampled probabilities are not multiples of 1/1024 (" + std::to_string(inexact) + " values): exact quantiles impossible");
+    sc.keep = keep;
+    return sample_histogram(bam, ctx, sc);
 }
 
 inline int run_summary(const SampleOptions& o, std::string* text, std::string* error) {
@@ -1631,54 +1459,18 @@ inline int run_summary(const SampleOptions& o, std::string* text, std::string* e
         mkp_params P;
         Region region; bool have_region = false;
         IncludeBed include; bool have_include = false;
-        std::vector<uint64_t> hist;
-        std::vector<SampledChunk> keep;
-        size_t n_selected = 0;
-        uint64_t inexact = 0;
-        sample_for_summary(o, dev.ctx, bam, &P, &region, &have_region, &include, &have_include, &hist, &keep, &n_selected, &inexact);
+        SampleResult sample = sample_for_summary(o, dev.ctx, true, bam, &P, &region, &have_region, &include, &have_include);
         ModSummaryOut S;
         // thresholds (src/commands.rs:1086-1098, 1147-1160)
-        for (auto& raw : o.mod_thresholds) {
-            auto c = raw.find(':');
-            uint32_t code;
-            if (c == std::string::npos || raw.find(':', c + 1) != std::string::npos || !parse_code(raw.substr(0, c), &code))
-                throw std::runtime_error("encountered illegal per-mod threshold: " + raw + ". Should be mod_code:threshold e.g. h:0.8");
-            if (P.n_mod_thresholds >= MKP_MAX_MOD_THRESHOLDS) throw std::runtime_error("too many per-mod thresholds");
-            P.mod_code[P.n_mod_thresholds] = code;
-            P.mod_threshold[P.n_mod_thresholds++] = std::stof(raw.substr(c + 1));
-        }
-        if (!o.filter_thresholds.empty()) {
-            bool have_default = false;
-            for (auto& raw : o.filter_thresholds) {
-                auto c = raw.find(':');
-                if (c == std::string::npos) { if (have_default) throw std::runtime_error("default threshold encountered more than once"); P.default_threshold = std::stof(raw); have_default = true; }
-                else {
-                    const char* B = "ACGT";
-                    const char* f = raw.empty() ? nullptr : strchr(B, raw[0]);
-                    if (!f || !raw[0]) throw std::runtime_error("failed to parse base " + raw);
-                    P.base_threshold_set[f - B] = 1;
-                    P.base_threshold[f - B] = std::stof(raw.substr(c + 1));
-                }
-            }
-        } else if (!o.no_filtering) {
-            require_exact(inexact);
-            for (int b = 0; b < 4; b++) {
-                uint64_t n = 0;
-                for (int k = 0; k < MKP_HIST_BINS; k++) n += hist[b * MKP_HIST_BINS + k];
-                if (!n) continue;
-                float thr;
-                if (!percentile_from_hist(hist.data() + b * MKP_HIST_BINS, o.percentile, &thr)) throw std::runtime_error("not enough datapoints to estimate a threshold");
-                P.base_threshold_set[b] = 1; P.base_threshold[b] = thr;
-            }
-        }
+        parse_mod_thresholds(o.mod_thresholds, &P);
+        parse_filter_thresholds(o.filter_thresholds, &P);
+        if (o.filter_thresholds.empty() && !o.no_filtering) estimated_thresholds(sample, o.percentile, "exact quantiles impossible", false, &P);
         for (int b = 0; b < 4; b++) { S.thresholds[b] = P.base_threshold[b]; S.threshold_set[b] = P.base_threshold_set[b]; }
         if (mkp_set_params(dev.ctx, &P)) throw std::runtime_error(mkp_last_error(dev.ctx));
         // ---- second pass over the sampled reads: counts per (base, state, pass / fail)
-        std::vector<uint32_t> fpos, fneg;
         const int incl_unal = !(o.only_mapped || have_include) ? 1 : 0;
-        for (auto& kc : keep) {
-            if (kc.pc.recs.empty()) continue;
-            upload_sample_chunk(dev.ctx, kc.pc, kc.tid, have_include ? &include : nullptr, &fpos, &fneg);
+        for (auto& kc : sample.keep) {
+            upload_sampled(bam, dev.ctx, kc.pc, kc.tid, have_include ? &include : nullptr);
             std::vector<uint64_t> table(4 * 2 * 33, 0), states(32, ~0ull);
             uint64_t rw[4] = {0, 0, 0, 0};
             uint32_t obs[4] = {0, 0, 0, 0};
@@ -1771,11 +1563,9 @@ inline int run_sample_probs(const SampleOptions& o, std::string* text, std::stri
         mkp_params P;
         Region region; bool have_region = false;
         IncludeBed include; bool have_include = false;
-        std::vector<uint64_t> hist;
-        size_t n_selected = 0;
-        uint64_t inexact = 0;
-        sample_for_summary(o, dev.ctx, bam, &P, &region, &have_region, &include, &have_include, &hist, nullptr, &n_selected, &inexact);
-        require_exact(inexact);
+        const SampleResult sample = sample_for_summary(o, dev.ctx, false, bam, &P, &region, &have_region, &include, &have_include);
+        require_exact(sample.inexact, "exact quantiles impossible");
+        const std::vector<uint64_t>& hist = sample.hist;
         std::vector<std::vector<std::string>> rows;
         rows.push_back({"base", "percentile", "threshold"});
         for (int b = 0; b < 4; b++) {
