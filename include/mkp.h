@@ -188,6 +188,13 @@ int  mkp_sample_histogram_wide(mkp_ctx* ctx, int include_unaligned, const uint8_
 int  mkp_sample_summary(mkp_ctx* ctx, int include_unaligned, const uint8_t* take, uint64_t* table, uint64_t* reads_with,
                         uint32_t* obs, uint64_t* states);
 
+/* `modkit sample-probs --hist` support: the calls of the reads flagged in `take` (every read if null), each counted under its
+ * arg-max call and the quality bin of the arg-max value (prob_to_qual: exactly 1.0 -> 255, else floor(p * 256) saturated to
+ * 0..255). Adds to hist (u64[4][33][256]: canonical base A C G T, 0 = canonical or 1 + state id, bin); inferred entries of
+ * implicit lists count as canonical in bin 255. states (u64[32]) receives the key of every state id of THIS call, as in
+ * mkp_sample_summary. */
+int  mkp_sample_mod_histogram(mkp_ctx* ctx, int include_unaligned, const uint8_t* take, uint64_t* hist, uint64_t* states);
+
 /* ---- BGZF / BAM ingest on the device (SURVEY §8f-1: the on-disk format step directly before the path) ----------
  * Replaces, for the records the path consumes, htslib's bgzf_read_block + inflate + bam_read1 behind
  * rust-htslib's bam::IndexedReader::{from_path, fetch} (src/pileup/mod.rs:732-743) and the tag lookup of

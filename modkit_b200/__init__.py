@@ -56,7 +56,7 @@ assert HEMI_ROW_DTYPE.itemsize == 44
 HIST_BINS = 2049        # MKP_HIST_BINS (include/mkp.h): bins k/1024 of mkp_sample_histogram_wide
 
 MKP_SYMBOLS = ["mkp_create", "mkp_bind_host_thread", "mkp_destroy", "mkp_last_error", "mkp_set_params", "mkp_upload_chunk", "mkp_pileup_resident",
-               "mkp_fetch_rows", "mkp_pileup_chunk", "mkp_sample_histogram", "mkp_sample_histogram_wide", "mkp_sample_summary", "mkp_algorithmic_bytes", "mkp_kernel_launches",
+               "mkp_fetch_rows", "mkp_pileup_chunk", "mkp_sample_histogram", "mkp_sample_histogram_wide", "mkp_sample_summary", "mkp_sample_mod_histogram", "mkp_algorithmic_bytes", "mkp_kernel_launches",
                "mkp_device_memory", "mkp_bam_load", "mkp_bam_load_range", "mkp_bam_load_range_fd", "mkp_bam_records", "mkp_bam_chunk", "mkp_bam_tags", "mkp_bam_inflated", "mkp_fetch_chunk",
                "mkp_hemi_resident", "mkp_fetch_hemi_rows"]
 MKH_SYMBOLS = ["mkh_pileup_main", "mkh_bam_open", "mkh_bam_close", "mkh_bam_n_refs", "mkh_bam_ref_name", "mkh_bam_ref_len",
@@ -65,7 +65,7 @@ MKH_SYMBOLS = ["mkh_pileup_main", "mkh_bam_open", "mkh_bam_close", "mkh_bam_n_re
                "mkh_motif_focus", "mkh_bam_open_device", "mkh_device_chunk", "mkh_bam_ingest_ms", "mkh_bam_total_records",
                "mkh_f32_display", "mkh_bam_partition_key", "mkh_bam_n_ranges", "mkh_pileup_main_sharded", "mkh_shard_plan",
                "mkh_bam_open_device_pieces", "mkh_bam_fetch", "mkh_summary_main", "mkh_sample_probs_main", "mkh_partition_key_of_cells", "mkh_bam_index_n_mapped", "mkh_pct2",
-               "mkh_pileup_hemi_main", "mkh_pileup_hemi_main_sharded"]
+               "mkh_pileup_hemi_main", "mkh_pileup_hemi_main_sharded", "mkh_probabilities_tsv"]
 
 ALLREDUCE_FN = C.CFUNCTYPE(C.c_int, C.POINTER(C.c_uint64), C.c_size_t, C.c_void_p)
 
@@ -102,6 +102,9 @@ def load_library(build_if_missing=True):
     lib.mkp_sample_histogram.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
     lib.mkp_sample_histogram_wide.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
     lib.mkp_sample_summary.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.mkp_sample_mod_histogram.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.mkh_probabilities_tsv.argtypes = [C.c_void_p, C.c_void_p, C.c_char_p, C.c_uint64]
+    lib.mkh_probabilities_tsv.restype = C.c_uint64
     lib.mkp_algorithmic_bytes.argtypes = [C.POINTER(Chunk), C.c_size_t]
     lib.mkp_algorithmic_bytes.restype = C.c_size_t
     lib.mkp_kernel_launches.argtypes = [C.c_void_p]
@@ -251,6 +254,18 @@ def pct2(v):
     if n < 0:
         raise MkpError("pct2 failed")
     return buf.value.decode()
+
+
+def probabilities_tsv(hist, states):
+    """`sample-probs --hist`'s probabilities.tsv of a (4, 33, 256) u64 histogram and its 32 state keys, as the host formats it
+    (CPU only)."""
+    lib = load_library()
+    h = np.ascontiguousarray(hist, dtype=np.uint64).reshape(4, 33, 256)
+    st = np.ascontiguousarray(states, dtype=np.uint64).reshape(32)
+    n = lib.mkh_probabilities_tsv(h.ctypes.data, st.ctypes.data, None, 0)
+    buf = C.create_string_buffer(n + 1)
+    lib.mkh_probabilities_tsv(h.ctypes.data, st.ctypes.data, buf, n)
+    return buf.raw[:n].decode()
 
 
 def bam_index_n_mapped(bam_path, tid):
@@ -536,6 +551,18 @@ class Context:
         self._check(fn(self._h, 1 if include_unaligned else 0, take_p, hist.ctypes.data,
                        contrib.ctypes.data if contrib is not None else None, C.byref(inexact)))
         return hist, contrib, inexact.value
+
+    def sample_mod_histogram(self, include_unaligned=False, take=None):
+        """(hist, states) of mkp_sample_mod_histogram: hist[base][s][qual] counts the arg-max calls, s = 0 canonical or 1 + state
+        id, qual = prob_to_qual of the arg-max value; states[id] = base << 32 | code of each state id (~0 unused)."""
+        hist = np.zeros((4, 33, 256), dtype=np.uint64)
+        states = np.full(32, 0xffffffffffffffff, dtype=np.uint64)
+        take_p = None
+        if take is not None:
+            take = np.ascontiguousarray(take, dtype=np.uint8)
+            take_p = take.ctypes.data
+        self._check(self._lib.mkp_sample_mod_histogram(self._h, 1 if include_unaligned else 0, take_p, hist.ctypes.data, states.ctypes.data))
+        return hist, states
 
     _n_reads_hint = 0
 

@@ -28,7 +28,8 @@ int mkh_pileup_hemi_main(int argc, const char* const* argv) {
     return 0;
 }
 
-// In-process `modkit summary` / `modkit sample-probs` (SURVEY 8f-3): the report goes to stdout, or to --out FILE.
+// In-process `modkit summary` / `modkit sample-probs` (SURVEY 8f-3): the report goes to stdout, or to --out FILE (sample-probs -o
+// DIR writes its files itself and leaves `text` empty).
 static int sample_main(int argc, const char* const* argv, bool summary) {
     SampleOptions o;
     std::string err, out_path, text;
@@ -148,6 +149,15 @@ uint64_t mkh_bam_total_records(const mkh_bam* b) { uint64_t n = b->reader.unplac
 // host-side helpers of --partition-tag / --bedgraph, exposed for the CPU tests
 int mkh_f32_display(float v, char* out, int cap) { const std::string s = f32_display(v); if ((int)s.size() + 1 > cap) return -1; memcpy(out, s.c_str(), s.size() + 1); return (int)s.size(); }
 int mkh_pct2(float v, char* out, int cap) { char b[64]; char* e = put_pct2(b, v); const int n = (int)(e - b); if (n + 1 > cap) return -1; memcpy(out, b, n); out[n] = 0; return n; }
+// sample-probs --hist: probabilities.tsv of one mkp_sample_mod_histogram result (hist u64[4][33][256], states u64[32]); returns the
+// text's length (copied to out when it fits in cap)
+uint64_t mkh_probabilities_tsv(const uint64_t* hist, const uint64_t* states, char* out, uint64_t cap) {
+    ModHistogram H;
+    add_mod_histogram(hist, states, &H);
+    const std::string text = probabilities_tsv(H);
+    if (out && text.size() <= cap) memcpy(out, text.data(), text.size());
+    return text.size();
+}
 // partition key of the i-th record of tid (file order) for the ':'-separated tag list; returns 1 key, 0 NoKey, -1 error
 int mkh_bam_partition_key(const mkh_bam* b, uint32_t tid, uint64_t i, const char* tags, char* out, int cap) {
     try {

@@ -1400,6 +1400,10 @@ struct SampleOptions {
     bool have_frac = false, no_sampling = false, no_filtering = false, only_mapped = false, invert_edge = false, tsv = false;
     double frac = 0;
     float percentile = 0.1f;
+    // sample-probs -o DIR: the report as files (thresholds.tsv; with --hist also probabilities.tsv, counts.html, proportion.html)
+    std::string out_dir, prefix;
+    bool have_prefix = false, force = false, hist = false;
+    std::vector<std::string> dna_colors, mod_colors;    // --dna-color / --mod-color values, two per occurrence
 };
 
 struct ModSummaryOut {
@@ -1546,9 +1550,167 @@ inline int run_summary(const SampleOptions& o, std::string* text, std::string* e
     } catch (const std::exception& e) { if (error) *error = e.what(); return 1; }
 }
 
-// `modkit sample-probs`: percentiles of the arg-max probabilities per canonical base (thresholds table, src/writers.rs:779-790)
+// ---- `sample-probs -o DIR [--hist]` (src/writers.rs:692-993, src/read_ids_to_base_mod_probs.rs:104-187) ----------------------
+// Counts of the arg-max values per (canonical base, state) and prob_to_qual bin. Key: (base, 0 = canonical | state_order_key),
+// so the map iterates in the reference's (DnaBase, BaseState) order: Canonical first, then Code(char) before ChEbi(u32).
+using ModHistogram = std::map<std::pair<int, uint64_t>, std::array<uint64_t, 256>>;
+
+// adds one mkp_sample_mod_histogram result (hist u64[4][33][256], states u64[32]) to H
+inline void add_mod_histogram(const uint64_t* hist, const uint64_t* states, ModHistogram* H) {
+    for (int b = 0; b < 4; b++) for (int s = 0; s < 33; s++) {
+        const uint64_t* h = hist + (b * 33 + s) * 256;
+        if (std::all_of(h, h + 256, [](uint64_t v) { return v == 0; })) continue;
+        std::array<uint64_t, 256>& dst = (*H)[{b, s == 0 ? 0 : state_order_key((uint32_t)states[s - 1])}];
+        for (int q = 0; q < 256; q++) dst[q] += h[q];
+    }
+}
+
+// probabilities.tsv (ProbHistogram::get_artifacts, src/writers.rs:837-945, csv writer with a tab delimiter): non-zero bins in
+// ascending order; frac and percentile_rank in f32, the rank over an f32 running sum of the counts, as the reference folds it
+inline std::string probabilities_tsv(const ModHistogram& H) {
+    std::string out = "code\tprimary_base\trange_start\trange_end\tcount\tfrac\tpercentile_rank\n";
+    for (const auto& kv : H) {
+        const std::array<uint64_t, 256>& c = kv.second;
+        uint64_t sum = 0;
+        for (uint64_t n : c) sum += n;
+        const float total = (float)sum;
+        const std::string head = (kv.first.second == 0 ? std::string("-") : state_label_of_key(kv.first.second)) + "\t" + "ACGT"[kv.first.first] + "\t";
+        float cum = 0.f;
+        for (int q = 0; q < 256; q++) {
+            if (!c[q]) continue;
+            const float n = (float)c[q];
+            cum = cum + n;
+            const float rank = ((cum - 0.5f * n) / total) * 100.0f;
+            out += head + f32_display((float)q / 256.0f) + "\t" + f32_display((float)(q + 1) / 256.0f) + "\t" + std::to_string(c[q]) + "\t" +
+                   f32_display(n / total) + "\t" + f32_display(rank) + "\n";
+        }
+    }
+    return out;
+}
+
+// JSON string literal, with '<' escaped so that a label or colour cannot close the page's <script>
+inline std::string json_str(const std::string& s) {
+    std::string o = "\"";
+    for (unsigned char ch : s) {
+        if (ch == '"' || ch == '\\') { o += '\\'; o += (char)ch; }
+        else if (ch < 0x20 || ch == '<') { char b[8]; snprintf(b, sizeof b, "\\u%04x", ch); o += b; }
+        else o += (char)ch;
+    }
+    return o + "\"";
+}
+
+// series colours: --dna-color / --mod-color, then the reference's defaults (mod_base_code.rs:94-102); any other label gets a
+// fixed colour derived from the label (FNV-1a), where the reference seeds the random_color crate with it
+struct HistColors { std::map<int, std::string> dna; std::map<uint32_t, std::string> mod; };
+
+inline HistColors parse_hist_colors(const SampleOptions& o) {
+    HistColors hc;
+    for (size_t i = 0; i + 1 < o.dna_colors.size(); i += 2) {
+        const std::string& b = o.dna_colors[i];
+        if (b.size() != 1) throw std::runtime_error("DNA base should be a char, " + b);
+        const char* f = strchr("ACGT", b[0]);
+        if (!f || !b[0]) throw std::runtime_error("invalid DNA base, should be A, C, G, or T: " + b);
+        hc.dna[(int)(f - "ACGT")] = o.dna_colors[i + 1];
+    }
+    for (size_t i = 0; i + 1 < o.mod_colors.size(); i += 2) {
+        uint32_t c;
+        if (!parse_code(o.mod_colors[i], &c)) throw std::runtime_error("failed to parse mod code " + o.mod_colors[i]);
+        hc.mod[c] = o.mod_colors[i + 1];
+    }
+    return hc;
+}
+
+inline std::string hist_series_color(const HistColors& hc, int base, uint64_t key, const std::string& label) {
+    if (key == 0) {
+        auto it = hc.dna.find(base);
+        if (it != hc.dna.end()) return it->second;
+        if (base == 1) return "#0000FF";
+        if (base == 0) return "#009600";
+    } else if (key < (1ull << 32)) {
+        const uint32_t code = (uint32_t)(key - 1);
+        auto it = hc.mod.find(code);
+        if (it != hc.mod.end()) return it->second;
+        if (code == 'm') return "#FF0000";
+        if (code == 'h') return "#FF00FF";
+        if (code == 'a') return "#0084A9";
+    } else {
+        auto it = hc.mod.find(0x80000000u | (uint32_t)(key - 1 - (1ull << 32)));
+        if (it != hc.mod.end()) return it->second;
+    }
+    uint32_t h = 2166136261u;
+    for (unsigned char ch : label) { h ^= ch; h *= 16777619u; }
+    char b[8];
+    snprintf(b, sizeof b, "#%06X", h & 0xffffffu);
+    return b;
+}
+
+// counts.html / proportion.html: one ECharts bar chart (get_blank_chart / get_artifacts, src/writers.rs:799-945) whose option
+// object is embedded as JSON, 800 x 800, ECharts loaded by <script src> as charming's HtmlRenderer does
+inline std::string histogram_chart_html(const ModHistogram& H, const HistColors& hc, bool proportion) {
+    std::vector<int> bins;
+    for (int q = 0; q < 256; q++) for (const auto& kv : H) if (kv.second[q]) { bins.push_back(q); break; }
+    std::string cats, series, colors;
+    for (int q : bins) {
+        char a[64], b[64];
+        *put_pct2(a, (float)q / 256.0f * 100.0f) = 0;
+        *put_pct2(b, (float)(q + 1) / 256.0f * 100.0f) = 0;
+        cats += std::string(cats.empty() ? "" : ",") + json_str(std::string("[") + a + ", " + b + ")");
+    }
+    for (const auto& kv : H) {
+        const int base = kv.first.first;
+        const std::string label = std::string(1, "ACGT"[base]) + ":" + (kv.first.second == 0 ? std::string("-") : state_label_of_key(kv.first.second));
+        int64_t tot = 0;
+        for (int q : bins) tot += (int64_t)kv.second[q];
+        std::string data;
+        for (int q : bins) {
+            const int64_t n = (int64_t)kv.second[q];
+            data += std::string(data.empty() ? "" : ",") + (proportion ? f32_display((float)n / (float)tot) : std::to_string(n));
+        }
+        series += std::string(series.empty() ? "" : ",") + "{\"type\":\"bar\",\"name\":" + json_str(label) + ",\"data\":[" + data + "]}";
+        colors += std::string(colors.empty() ? "" : ",") + json_str(hist_series_color(hc, base, kv.first.second, label));
+    }
+    const char* title = proportion ? "Proportion" : "Counts";
+    const std::string option = std::string("{\"title\":{\"text\":\"") + title + "\"},\"tooltip\":{\"trigger\":\"axis\",\"axisPointer\":{\"type\":\"shadow\"}},"
+        "\"legend\":{},\"toolbox\":{\"feature\":{\"dataZoom\":{\"yAxisIndex\":\"none\"},\"restore\":{},\"saveAsImage\":{}}},"
+        "\"dataZoom\":[{\"type\":\"slider\"}],\"xAxis\":{\"type\":\"category\",\"name\":\"bin\",\"data\":[" + cats + "]},"
+        "\"yAxis\":{\"type\":\"value\",\"name\":\"" + (proportion ? "proportion" : "counts") + "\"},\"color\":[" + colors + "],\"series\":[" + series + "]}";
+    return std::string("<!DOCTYPE html>\n<html lang=\"en\">\n<head>\n  <meta charset=\"utf-8\">\n  <title>") + (proportion ? "Proportions" : "Counts") +
+           "</title>\n  <script src=\"https://cdn.jsdelivr.net/npm/echarts@5.4.2/dist/echarts.min.js\"></script>\n</head>\n<body>\n"
+           "  <div id=\"chart\" style=\"width:800px;height:800px;\"></div>\n  <script type=\"text/javascript\">\n"
+           "    var option = " + option + ";\n"
+           "    echarts.init(document.getElementById(\"chart\")).setOption(option);\n  </script>\n</body>\n</html>\n";
+}
+
+// the files of `-o DIR` (SampledProbs::get_*_filename*, src/writers.rs:700-725)
+inline std::vector<std::string> sample_output_files(const SampleOptions& o) {
+    const std::string p = o.have_prefix ? o.prefix + "_" : "";
+    std::vector<std::string> v{p + "thresholds.tsv"};
+    if (o.hist) for (const char* n : {"probabilities.tsv", "counts.html", "proportion.html"}) v.push_back(p + n);
+    return v;
+}
+
+// SampledProbs::check_files (src/writers.rs:731-763) and the colour arguments: before any device work or sampling
+inline HistColors check_sample_outputs(const SampleOptions& o) {
+    if (o.out_dir.empty()) return HistColors();
+    for (const std::string& n : sample_output_files(o)) {
+        const std::filesystem::path fp = std::filesystem::path(o.out_dir) / n;
+        if (std::filesystem::exists(fp) && !o.force) throw std::runtime_error("refusing to overwrite \"" + fp.string() + "\"");
+    }
+    return parse_hist_colors(o);
+}
+
+inline void write_text_file(const std::filesystem::path& fp, const std::string& text) {
+    FILE* f = fopen(fp.c_str(), "wb");
+    if (!f) throw std::runtime_error("failed to create " + fp.string());
+    const bool ok = fwrite(text.data(), 1, text.size(), f) == text.size();
+    if (fclose(f) != 0 || !ok) throw std::runtime_error("failed to write " + fp.string());
+}
+
+// `modkit sample-probs`: percentiles of the arg-max probabilities per canonical base (thresholds table, src/writers.rs:779-790);
+// with -o the table goes to DIR/thresholds.tsv and nothing to stdout, with --hist also the per-state histograms
 inline int run_sample_probs(const SampleOptions& o, std::string* text, std::string* error) {
     try {
+        const HistColors colors = check_sample_outputs(o);
         DeviceGuard dev;
         { const int rc = mkp_create(o.device, &dev.ctx); if (rc) throw std::runtime_error("no usable CUDA device (mkp_create returned " + std::to_string(rc) + "); this build has no CPU fallback"); }
         std::vector<float> qs;
@@ -1563,7 +1725,7 @@ inline int run_sample_probs(const SampleOptions& o, std::string* text, std::stri
         mkp_params P;
         Region region; bool have_region = false;
         IncludeBed include; bool have_include = false;
-        const SampleResult sample = sample_for_summary(o, dev.ctx, false, bam, &P, &region, &have_region, &include, &have_include);
+        SampleResult sample = sample_for_summary(o, dev.ctx, o.hist, bam, &P, &region, &have_region, &include, &have_include);
         require_exact(sample.inexact, "exact quantiles impossible");
         const std::vector<uint64_t>& hist = sample.hist;
         std::vector<std::vector<std::string>> rows;
@@ -1583,6 +1745,28 @@ inline int run_sample_probs(const SampleOptions& o, std::string* text, std::stri
         for (auto& r : rows) for (size_t i = 0; i < 3; i++) w[i] = std::max(w[i], r[i].size());
         text->clear();
         for (auto& r : rows) { for (size_t i = 0; i < 3; i++) { *text += " " + r[i] + std::string(w[i] - r[i].size(), ' ') + " "; } *text += "\n"; }
+        if (o.out_dir.empty()) return 0;
+        // ---- -o DIR: the histograms are a second device pass over the sampled reads (get_per_mod_histograms)
+        ModHistogram H;
+        if (o.hist) {
+            const int incl_unal = !(o.only_mapped || have_include) ? 1 : 0;
+            for (auto& kc : sample.keep) {
+                upload_sampled(bam, dev.ctx, kc.pc, kc.tid, have_include ? &include : nullptr);
+                std::vector<uint64_t> hist(4 * 33 * 256, 0), states(32, ~0ull);
+                if (mkp_sample_mod_histogram(dev.ctx, incl_unal, kc.take.data(), hist.data(), states.data())) throw std::runtime_error(mkp_last_error(dev.ctx));
+                add_mod_histogram(hist.data(), states.data(), &H);
+            }
+        }
+        const std::filesystem::path dir(o.out_dir);
+        std::filesystem::create_directories(dir);
+        const std::vector<std::string> files = sample_output_files(o);
+        write_text_file(dir / files[0], *text);
+        if (o.hist) {
+            write_text_file(dir / files[1], probabilities_tsv(H));
+            write_text_file(dir / files[2], histogram_chart_html(H, colors, false));
+            write_text_file(dir / files[3], histogram_chart_html(H, colors, true));
+        }
+        text->clear();
         return 0;
     } catch (const std::exception& e) { if (error) *error = e.what(); return 1; }
 }
@@ -1615,12 +1799,25 @@ inline bool parse_sample_args(int argc, const char* const* argv, bool summary, S
             else if (summary && a == "--tsv") o->tsv = true;
             else if (summary && a == "--table") o->tsv = false;
             else if (!summary && (a == "-p" || a == "--percentiles")) o->percentiles = val();
-            else if (!summary && (a == "--hist" || a == "-o" || a == "--out-dir" || a == "--prefix" || a == "--force" || a == "--dna-color" || a == "--mod-color"))
-                throw std::runtime_error("histogram / file outputs of sample-probs (" + a + ") are not provided by this build: the percentile table goes to stdout");
+            else if (!summary && (a == "-o" || a == "--out-dir")) o->out_dir = val();
+            else if (!summary && a == "--prefix") { o->prefix = val(); o->have_prefix = true; }
+            else if (!summary && a == "--force") o->force = true;
+            else if (!summary && a == "--hist") o->hist = true;
+            else if (!summary && (a == "--dna-color" || a == "--mod-color")) {
+                std::vector<std::string>& v = a == "--dna-color" ? o->dna_colors : o->mod_colors;
+                if (i + 2 >= argc) throw std::runtime_error("invalid number of arguments for '" + a + "': 2 values are required");
+                v.push_back(argv[++i]);
+                v.push_back(argv[++i]);
+            }
             else if (a.size() > 1 && a[0] == '-') { *err = "unexpected argument '" + a + "' found"; return false; }
             else pos.push_back(a);
         } catch (const std::exception& e) { *err = e.what(); return false; }
     }
+    // the `requires` rules of the output flags (src/commands.rs:573-622); --out is this build's report file, -o the reference's directory
+    const char* needs_out_dir = o->have_prefix ? "--prefix" : o->force ? "--force" : o->hist ? "--hist" : nullptr;
+    if (needs_out_dir && o->out_dir.empty()) { *err = std::string("the following required arguments were not provided: --out-dir <OUT_DIR> (required by ") + needs_out_dir + ")"; return false; }
+    if (!o->hist && !(o->dna_colors.empty() && o->mod_colors.empty())) { *err = "the following required arguments were not provided: --hist (required by --dna-color / --mod-color)"; return false; }
+    if (!o->out_dir.empty() && !out_path->empty()) { *err = "the argument '--out <FILE>' cannot be used with '--out-dir <OUT_DIR>'"; return false; }
     if (pos.size() != 1) { *err = "the following required arguments were not provided: <IN_BAM>"; return false; }
     o->in_bam = pos[0];
     return true;

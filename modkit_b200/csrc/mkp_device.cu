@@ -756,9 +756,11 @@ int mkp_pileup_chunk(mkp_ctx* ctx, const mkp_chunk* ch, const mkp_row** rows, si
 }
 
 // The sampling decode (MODE_HIST) of the resident chunk, over the reads flagged in `take` (every read if null). `out_words` u64
-// counters at d_hist are zeroed and attached as C.summ (`summary`) or C.hist; none if 0. The caller enqueues its copies back,
-// then finish_status.
-static int sample_decode(mkp_ctx* ctx, int include_unaligned, const uint8_t* take, bool summary, size_t out_words) {
+// counters at d_hist are zeroed and attached as C.summ, C.qhist or C.hist (by `out`); none if 0. The caller enqueues its copies
+// back, then finish_status.
+enum SampleOut { OUT_HIST, OUT_SUMMARY, OUT_QHIST };
+static constexpr size_t QHIST_WORDS = 4 * 33 * 256;
+static int sample_decode(mkp_ctx* ctx, int include_unaligned, const uint8_t* take, SampleOut out, size_t out_words) {
     if (!ctx->have_params) return fail(ctx, "mkp_set_params was not called");
     if (ctx->ce <= ctx->cs) return fail(ctx, "no resident chunk");
     CK(cudaSetDevice(ctx->device));
@@ -774,9 +776,10 @@ static int sample_decode(mkp_ctx* ctx, int include_unaligned, const uint8_t* tak
         C.take = ctx->d_take.as<uint8_t>();
     }
     if (out_words) {
-        CK(ctx->d_hist.ensure(std::max<size_t>(4 * MKP_HIST_BINS, out_words) * 8));     // one size for both uses: no regrowth between them
+        CK(ctx->d_hist.ensure(std::max<size_t>(QHIST_WORDS, out_words) * 8));     // one size for every use: no regrowth between them
         CK(cudaMemsetAsync(ctx->d_hist.p, 0, out_words * 8, st));
-        if (summary) C.summ = ctx->d_hist.as<unsigned long long>();
+        if (out == OUT_SUMMARY) C.summ = ctx->d_hist.as<unsigned long long>();
+        else if (out == OUT_QHIST) C.qhist = ctx->d_hist.as<unsigned long long>();
         else C.hist = ctx->d_hist.as<unsigned long long>();
     }
     return decode(ctx, C, grid);
@@ -784,7 +787,7 @@ static int sample_decode(mkp_ctx* ctx, int include_unaligned, const uint8_t* tak
 
 int mkp_sample_histogram_wide(mkp_ctx* ctx, int include_unaligned, const uint8_t* take, uint64_t* hist, uint8_t* contributes, uint64_t* inexact) {
     if (!ctx) return -1;
-    if (int rc = sample_decode(ctx, include_unaligned, take, false, hist ? 4 * MKP_HIST_BINS : 0)) return rc;
+    if (int rc = sample_decode(ctx, include_unaligned, take, OUT_HIST, hist ? 4 * MKP_HIST_BINS : 0)) return rc;
     if (hist) CK(cudaMemcpyAsync(hist, ctx->d_hist.p, 4 * MKP_HIST_BINS * 8, cudaMemcpyDeviceToHost, ctx->stream));
     std::vector<ReadMeta> metas;
     if (contributes) {
@@ -817,7 +820,7 @@ int mkp_sample_histogram(mkp_ctx* ctx, int include_unaligned, const uint8_t* tak
 int mkp_sample_summary(mkp_ctx* ctx, int include_unaligned, const uint8_t* take, uint64_t* table, uint64_t* reads_with, uint32_t* obs, uint64_t* states) {
     if (!ctx || !table || !reads_with || !obs || !states) return -1;
     const size_t words = 4 * 2 * 33 + 4 + 2;
-    if (int rc = sample_decode(ctx, include_unaligned, take, true, words)) return rc;
+    if (int rc = sample_decode(ctx, include_unaligned, take, OUT_SUMMARY, words)) return rc;
     std::vector<uint64_t> hv(words);
     CK(cudaMemcpyAsync(hv.data(), ctx->d_hist.p, words * 8, cudaMemcpyDeviceToHost, ctx->stream));
     PassScratch h;
@@ -826,6 +829,20 @@ int mkp_sample_summary(mkp_ctx* ctx, int include_unaligned, const uint8_t* take,
     for (int b = 0; b < 4; b++) reads_with[b] += hv[4 * 2 * 33 + b];
     const uint32_t* o32 = (const uint32_t*)(hv.data() + 4 * 2 * 33 + 4);
     for (int b = 0; b < 4; b++) obs[b] = o32[b];
+    memcpy(states, h.states, sizeof h.states);
+    return 0;
+}
+
+// `modkit sample-probs --hist` support (src/read_ids_to_base_mod_probs.rs:104-187): adds to hist[4][33][256] (base, 0 canonical |
+// 1 + state id, prob_to_qual bin of the arg-max value); states[32] as in mkp_sample_summary.
+int mkp_sample_mod_histogram(mkp_ctx* ctx, int include_unaligned, const uint8_t* take, uint64_t* hist, uint64_t* states) {
+    if (!ctx || !hist || !states) return -1;
+    if (int rc = sample_decode(ctx, include_unaligned, take, OUT_QHIST, QHIST_WORDS)) return rc;
+    std::vector<uint64_t> hv(QHIST_WORDS);
+    CK(cudaMemcpyAsync(hv.data(), ctx->d_hist.p, QHIST_WORDS * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    PassScratch h;
+    if (int rc = finish_status(ctx, nullptr, &h)) return rc;
+    for (size_t i = 0; i < QHIST_WORDS; i++) hist[i] += hv[i];
     memcpy(states, h.states, sizeof h.states);
     return 0;
 }

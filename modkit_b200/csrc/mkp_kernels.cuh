@@ -100,6 +100,9 @@ struct ChunkDev {
     // by (thresholded call, arg-max call): summ[((base * 2 + fail) * 33) + s], s = 0 canonical, 1 + state id; then reads per base
     // [4] and, as u32, the states observed per base [4]. nullptr = off.
     unsigned long long* summ;
+    // `modkit sample-probs --hist` (src/read_ids_to_base_mod_probs.rs:104-187): every value of MODE_HIST counted under its
+    // arg-max call and prob_to_qual bin: qhist[(base * 33 + s) * 256 + qual], s = 0 canonical, 1 + state id. nullptr = off.
+    unsigned long long* qhist;
     uint32_t mode;              // MODE_PILEUP / MODE_HIST (admission rules of k_parse)
     struct ReadLists* rl;
     // chunks with focus bitmaps (the hot bitmap is the focus set, ranked at upload, and is not written):
@@ -113,6 +116,14 @@ struct ChunkDev {
 __constant__ DevParams c_par;
 
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
+
+// prob_to_qual (mod_bam.rs:798-806): exactly 1.0 -> 255, else floor(p * 256) in f32 with Rust's saturating `as u8` (NaN and
+// negatives -> 0, values from 255/256 up -> 255)
+__device__ __forceinline__ uint32_t prob_to_qual(float p) {
+    if (p == 1.0f) return 255u;
+    const float s = __fmul_rn(p, 256.0f);
+    return s >= 255.0f ? 255u : s > 0.0f ? (uint32_t)s : 0u;
+}
 
 __device__ __forceinline__ uint32_t warp_incl_scan(uint32_t v) {
 #pragma unroll
@@ -1104,6 +1115,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                     bool hist_ok = false;
                     float hist_v = 0.f;
                     int hist_base = 0;
+                    uint32_t hist_q = 0;
                     if (active) {
                         uint32_t f = Pl[j];
                         uint32_t q = rev ? L - 1u - f : f;
@@ -1221,7 +1233,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                                         if (n2c >= 1) { mp = p0; hm2 = true; }
                                         if (n2c == 2 && p1 >= mp) mp = p1;
                                         hv = (hm2 && mp > cp) ? mp : cp;
-                                        if (C.summ) {
+                                        if (C.summ || C.qhist) {
                                             // thresholded call (as in the pileup) and arg-max call (last maximum wins, mod_bam.rs:489-505)
                                             uint32_t s0 = 0, s1 = 0;
                                             if (n2c >= 1) { s0 = (uint32_t)state_id(C, scache, tb, c0); mask |= 1u << s0; }
@@ -1298,7 +1310,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                                     kind = make_call_items(*use, ord, tb, &ccode);
                                 } else {
                                     hv = argmax_items(*use, ord);
-                                    if (C.summ) {
+                                    if (C.summ || C.qhist) {
                                         uint32_t tcode = 0;
                                         const int tkind = make_call_items(*use, ord, tb, &tcode);
                                         uint32_t ts = 0, as = 0;
@@ -1371,7 +1383,8 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                                         }
                                         if (pass) {
                                             hist_ok = true; hist_v = hv; hist_base = tb;
-                                            if (C.summ) { hist_v = __uint_as_float(ccode); sum_obs[tb] |= mask; }
+                                            if (C.summ || C.qhist) { hist_q = prob_to_qual(hv); hist_v = __uint_as_float(ccode); }
+                                            if (C.summ) sum_obs[tb] |= mask;
                                             if (!FAST_ONLY && imp_lists[st][b]) imp_explicit[st * 4 + b]++;
                                         }
                                     }
@@ -1394,14 +1407,15 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                     } else {
                         uint32_t hm = __ballot_sync(FULL, hist_ok);
                         if (hist_ok) {
-                            // stash (bin | base<<16 | inexact<<20) in the call buffer; committed after validation. Values
-                            // above 1.0 are legal (ML sums up to 1.01, ReDistribute shares) and get their own bins
-                            float sc = __fmul_rn(C.summ ? 0.f : hist_v, 1024.0f);
+                            // stash (bin | base<<16 | inexact<<20 | qual<<21) in the call buffer; committed after validation.
+                            // Values above 1.0 are legal (ML sums up to 1.01, ReDistribute shares) and get their own bins.
+                            // With summ / qhist, y holds the packed classification and the bin is 0
+                            float sc = __fmul_rn((C.summ || C.qhist) ? 0.f : hist_v, 1024.0f);
                             int bin = (int)rintf(sc);
                             uint32_t inexact = ((float)bin != sc || bin < 0 || bin >= MKP_HIST_BINS) ? 1u : 0u;
                             if (bin < 0) bin = 0;
                             if (bin >= MKP_HIST_BINS) bin = MKP_HIST_BINS - 1;
-                            calls[n_hist + __popc(hm & ((1u << lane) - 1u))] = make_uint2((uint32_t)bin | ((uint32_t)hist_base << 16) | (inexact << 20), __float_as_uint(hist_v));
+                            calls[n_hist + __popc(hm & ((1u << lane) - 1u))] = make_uint2((uint32_t)bin | ((uint32_t)hist_base << 16) | (inexact << 20) | (hist_q << 21), __float_as_uint(hist_v));
                         }
                         n_hist += __popc(hm);
                     }
@@ -1560,6 +1574,18 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                             if ((seen >> b) & 1u) atomicAdd(&C.summ[4 * 2 * 33 + b], 1ull);
                             if (obs[b]) atomicOr((uint32_t*)(C.summ + 4 * 2 * 33 + 4) + b, obs[b]);
                         }
+                    }
+                }
+                if (C.qhist) {
+                    for (uint32_t k = lane; k < n_hist; k += 32) {
+                        const uint2 v = calls[k];
+                        const uint32_t tb = (v.x >> 16) & 3u, q = (v.x >> 21) & 255u, ak = (v.y >> 8) & 3u, as = (v.y >> 10) & 63u;
+                        atomicAdd(&C.qhist[(tb * 33 + (ak == 2 ? 1 + as : 0)) * 256 + q], 1ull);
+                    }
+                    // an inferred entry is the all-zero map: canonical with probability 1.0, qual 255
+                    if (lane == 0) for (int sb = 0; sb < 8; sb++) if (imp_hist[sb]) {
+                        const int tb = (sb >> 2) == 0 ? (sb & 3) : 3 - (sb & 3);
+                        atomicAdd(&C.qhist[(tb * 33 + 0) * 256 + 255], imp_hist[sb]);
                     }
                 }
                 if (C.hist) {
