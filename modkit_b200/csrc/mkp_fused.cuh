@@ -154,7 +154,7 @@ __device__ __forceinline__ void fz_lists_and_tokens(uint32_t* err_flags, FzWarp&
                         const uint8_t c = mm[k];
                         if (c == '?') mode = 0;
                         else if (c == '.') mode = 1;
-                        else if (is_digit(c) || seen_chebi) e = true;
+                        else if (is_digit(c) || seen_chebi || c >= 0x80) e = true;   // (a non-ASCII header is a read error)
                         else if (nc >= MAX_LIST_CODES) { atomicOr(F.err, MKP_DERR_TOO_MANY_CODES); e = true; }
                         else T.code[n][nc++] = c;
                     }
@@ -365,7 +365,7 @@ __device__ __forceinline__ void fz_lists_and_tokens(uint32_t* err_flags, FzWarp&
                     while (k < nvalid && is_ws(chr(k))) k++;
                     const uint32_t d0 = k;
                     while (k < nvalid && is_digit(chr(k))) { val = val * 10 + (chr(k) - '0'); if (val > 0xffffffffull) val = 0x1ffffffffull; k++; }
-                    ok_start = k > d0 && val <= 0xffffffffull;
+                    ok_start = k > d0;                                 // a number above u32 keeps its place (clamped to 2^33 - 1): place() fails the read
                     while (k < nvalid && is_ws(chr(k))) k++;
                     clean = (k >= nvalid) || (chr(k) == ',');
                 }

@@ -386,7 +386,7 @@ __device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t* P, uint32_t 
 
 // Kernel A: per read, everything that depends only on the read's own bytes: admission, reference span, MM list
 // discovery, per-base occurrence counts, MM token parse + select -> forward positions P[] and the list table.
-// k_parse: 9 blocks of 128 threads = 56 registers and no spills. At 10 blocks (48 registers) it spills 72 / 100 bytes and takes
+// k_parse: 9 blocks of 128 threads = a limit of 56 registers; it takes 55 and does not spill. At 10 blocks (48 registers) it spills 72 / 100 bytes and takes
 // 1.4 % longer on an H100; at 8 (63 registers, 32 warps per SM) it took 2 % longer (profiles/README.md)
 #ifndef MKP_MINB_PARSE
 #define MKP_MINB_PARSE 9
@@ -508,7 +508,7 @@ __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
                             const uint8_t c = mm[k];
                             if (c == '?') mode = 0;
                             else if (c == '.') mode = 1;
-                            else if (is_digit(c) || seen_chebi) e = true;
+                            else if (is_digit(c) || seen_chebi || c >= 0x80) e = true;   // (a non-ASCII header is a read error)
                             else if (nc >= MAX_LIST_CODES) { atomicOr(C.err, MKP_DERR_TOO_MANY_CODES); e = true; }
                             else T.code[n][nc++] = c;
                         }
@@ -738,7 +738,7 @@ __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
                         while (k < nvalid && is_ws(chr(k))) k++;
                         const uint32_t d0 = k;
                         while (k < nvalid && is_digit(chr(k))) { val = val * 10 + (chr(k) - '0'); if (val > 0xffffffffull) val = 0x1ffffffffull; k++; }
-                        ok_start = k > d0 && val <= 0xffffffffull;
+                        ok_start = k > d0;                                 // a number above u32 keeps its place (clamped to 2^33 - 1): place() fails the read
                         while (k < nvalid && is_ws(chr(k))) k++;
                         clean = (k >= nvalid) || (chr(k) == ',');
                     }

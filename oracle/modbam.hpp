@@ -24,7 +24,8 @@
 
 namespace orc {
 
-// ModCodeRepr as u32: Code(char) = code point; ChEbi(n) = 0x80000000 | n.
+// ModCodeRepr as u32: Code(char) = code point; ChEbi(n) = 0x80000000 | n, so n has 31 bits: a larger ChEBI number is an error
+// (a read error in an MM header), where the reference takes any u32.
 // Derived Ord (src/mod_base_code.rs:106): Code(_) < ChEbi(_), then by value  == plain u32 order.
 typedef uint32_t ModCode;
 inline bool code_is_chebi(ModCode c) { return c & 0x80000000u; }
@@ -36,7 +37,7 @@ inline bool parse_mod_code(const std::string& raw, ModCode* out) {  // ModCodeRe
     if (raw.size() == 1) { *out = (uint8_t)raw[0]; return true; }
     if (raw.empty()) return false;
     uint64_t v = 0;
-    for (char ch : raw) { if (ch < '0' || ch > '9') return false; v = v * 10 + (ch - '0'); if (v > 0xffffffffull) return false; }
+    for (char ch : raw) { if (ch < '0' || ch > '9') return false; v = v * 10 + (ch - '0'); if (v > 0x7fffffffull) return false; }
     *out = 0x80000000u | (uint32_t)v;
     return true;
 }
@@ -154,7 +155,7 @@ inline bool parse_mm(const char* s, size_t n, std::vector<MmList>* out) {
             int mode = -1;
             if (k < hlen && part[k] >= '0' && part[k] <= '9') {
                 uint64_t v = 0;
-                while (k < hlen && part[k] >= '0' && part[k] <= '9') { v = v * 10 + (part[k] - '0'); if (v > 0xffffffffull) return false; k++; }
+                while (k < hlen && part[k] >= '0' && part[k] <= '9') { v = v * 10 + (part[k] - '0'); if (v > 0x7fffffffull) return false; k++; }
                 L.codes.push_back(0x80000000u | (uint32_t)v);
                 seen_chebi = true;
             }
@@ -163,6 +164,7 @@ inline bool parse_mm(const char* s, size_t n, std::vector<MmList>* out) {
                 if (c == '?') mode = EXPLICIT;
                 else if (c == '.') mode = IMPLICIT;
                 else if (c >= '0' && c <= '9') return false;
+                else if ((uint8_t)c >= 0x80) return false;  // the reference splits at a character count: the delta text would start off place
                 else { if (seen_chebi) return false; L.codes.push_back((uint8_t)c); }
             }
             L.mode = mode < 0 ? DEFAULT_IMPLICIT : mode;
