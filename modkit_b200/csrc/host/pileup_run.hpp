@@ -12,6 +12,7 @@
 #include <functional>
 #include <future>
 #include <memory>
+#include <numeric>
 #include <filesystem>
 #include <optional>
 #include <set>
@@ -45,8 +46,7 @@ struct PileupOptions {
     bool hemi = false;                 // `modkit pileup-hemi`: duplex pattern counts at the + strand positions of one palindromic motif
 };
 
-// pileup-hemi's motif (src/pileup/subcommand.rs:1242-1272): exactly one, --cpg or --motif, and it must be a palindrome. Checked
-// before any device work, so argument errors need no GPU.
+// pileup-hemi's motif (src/pileup/subcommand.rs:1242-1272): exactly one, --cpg or --motif, and it must be a palindrome
 inline MotifSpec hemi_motif(const PileupOptions& o) {
     if (o.ref_fp.empty()) throw std::runtime_error("the following required arguments were not provided: --ref <REFERENCE_FASTA>");
     if (o.cpg && !o.motif_parts.empty()) throw std::runtime_error("the argument '--cpg' cannot be used with '--motif <MOTIF> <MOTIF>'");
@@ -655,7 +655,7 @@ struct RunSummary {
     uint64_t positions = 0, rows = 0, reads_packed = 0, algorithmic_bytes = 0, chunks = 0;
     uint64_t rows_total = 0, positions_total = 0;      // over all ranks of a sharded run
     double fetch_s = 0;                                // threshold sampler: host fetch of the candidates
-    double slice_s = 0, pass_s = 0, rowcopy_s = 0;     // parts of gpu_s: GPU slicing + upload of focus, kernels, rows to the host
+    double slice_s = 0, pass_s = 0, rowcopy_s = 0;     // parts of gpu_s: making the chunk resident (GPU slicing or upload), kernels, rows to the host
     double load_s = 0, threshold_s = 0, interval_s = 0, pack_s = 0, gpu_s = 0, write_s = 0, total_s = 0, kernel_ms = 0;
     float thresholds[4] = {0, 0, 0, 0};
     bool threshold_set[4] = {false, false, false, false};
@@ -684,64 +684,61 @@ inline std::vector<size_t> shard_cuts(const BamReader& bam, const std::vector<Re
     return cuts;
 }
 
-inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* error, const Collective* coll_in = nullptr) {
-    using clk = std::chrono::steady_clock;
-    auto secs = [](clk::time_point a, clk::time_point b) { return std::chrono::duration<double>(b - a).count(); };
-    const Collective coll = coll_in ? *coll_in : Collective();
-    const bool sharded = coll.world > 1;
-    try {
-        const auto t0 = clk::now();
-        trace_clock().epoch = t0;
-        auto trace = [&](const char* what) { trace_clock().mark(coll.rank, what); };
+// the context of CUDA device `device`; this build has no CPU fallback, so a machine without a usable device stops here
+inline mkp_ctx* open_device(int device) {
+    mkp_ctx* ctx = nullptr;
+    if (const int rc = mkp_create(device, &ctx)) throw std::runtime_error("no usable CUDA device (mkp_create returned " + std::to_string(rc) + "); this build has no CPU fallback");
+    return ctx;
+}
+inline void check_mkp(mkp_ctx* ctx, int rc) { if (rc) throw std::runtime_error(mkp_last_error(ctx)); }
+
+// A job on a thread of its own. An exception it throws is kept and rethrown by join(). `release` (optional) runs on the owner's
+// thread before the join, to let go a job that may be waiting on the owner. Declare the job after every object it touches, so
+// that it is destroyed (joined) before they are.
+class BackgroundJob {
+    std::function<void()> release_;
+    std::exception_ptr err_;
+    std::thread t_;
+public:
+    explicit BackgroundJob(std::function<void()> fn, std::function<void()> release = nullptr)
+        : release_(std::move(release)), t_([this, fn = std::move(fn)]() { try { fn(); } catch (...) { err_ = std::current_exception(); } }) {}
+    ~BackgroundJob() { if (t_.joinable()) { if (release_) release_(); t_.join(); } }
+    void join() { if (release_) release_(); t_.join(); if (err_) std::rethrow_exception(err_); }
+};
+
+// What a pileup run needs from its options. The constructor makes every check that needs no device and no file, in the
+// reference's order, so argument errors need no GPU; open_inputs and lay_out follow once the BAM header is read.
+struct PileupPlan {
+    mkp_params P{};                    // the thresholds are added once the output exists (subcommand.rs:615-638)
+    MotifContext mc;
+    BedFormat fmt;
+    bool have_motifs = false, combine_strands = false;
+    bool to_dir = false;               // the output path is a directory (writers.rs:264-381, 1005-1082)
+    int32_t hemi_partner = 0;          // pileup-hemi: MotifInfo::negative_strand_position
+    std::optional<Region> region, sregion;
+    std::vector<RefTarget> targets, iv_targets;
+    IncludeBed include;
+    const IncludeBed* inc = nullptr;
+    std::vector<RefInterval> ivs;
+    std::vector<size_t> iv_owner;
+    size_t my_i0 = 0, my_i1 = 0;       // this rank's intervals
+    PileupPlan(const PileupPlan&) = delete;
+    PileupPlan(const PileupOptions& o, bool sharded) {
         if (o.percentile > 1.0f) throw std::runtime_error("filter percentile must be <= 1.0");
         MotifSpec hemi_m;
-        if (o.hemi) hemi_m = hemi_motif(o);
-        const int32_t hemi_partner = o.hemi ? hemi_m.rc_offset - hemi_m.offset : 0;     // MotifInfo::negative_strand_position
-        // the device comes first: with the device ingest (default) the BAM is inflated and sliced on the GPU
-        DeviceGuard dev;
-        {
-            const int rc = mkp_create(o.device, &dev.ctx);
-            if (rc) throw std::runtime_error("no usable CUDA device (mkp_create returned " + std::to_string(rc) + "); this build has no CPU fallback");
-        }
-        trace("device context created");
-        BamReader bam;
+        if (o.hemi) { hemi_m = hemi_motif(o); hemi_partner = hemi_m.rc_offset - hemi_m.offset; }
         // util.rs:690-712
         for (size_t i = 0; i < o.partition_tags.size(); i++) {
             if (o.partition_tags[i].size() != 2) throw std::runtime_error("illegal tag " + o.partition_tags[i] + " should be length 2");
             for (size_t j = 0; j < i; j++) if (o.partition_tags[j] == o.partition_tags[i]) throw std::runtime_error("cannot repeat partition-tags, got " + o.partition_tags[i] + " twice");
         }
-        const bool partitioned = !o.partition_tags.empty();
-        const bool to_dir = partitioned || o.bedgraph;     // the output path is a directory (writers.rs:264-381, 1005-1082)
+        to_dir = !o.partition_tags.empty() || o.bedgraph;
         if (to_dir && o.header) throw std::runtime_error("the argument '--header' cannot be used with '--bedgraph' / '--partition-tag'");
         if (o.bedgraph && o.mixed) throw std::runtime_error("the argument '--mixed-delim' cannot be used with '--bedgraph'");
         if (sharded && (to_dir || o.host_ingest)) throw std::runtime_error("multi-GPU runs write one bedMethyl file through the device ingest: --bedgraph / --partition-tag / --host-ingest need a single device");
         if (sharded && (o.out_bed == "-" || o.out_bed == "stdout")) throw std::runtime_error("multi-GPU runs need an output file (ranks write their slices at their offsets)");
-        // (partition keys: the tag values come from the device-resident records, mkp_bam_tags; --host-ingest reads them on the host)
-        bool loaded = false;
-        if (o.host_ingest) { bam.open(o.in_bam, o.threads); loaded = true; }
-        else bam.open_device_index(o.in_bam, dev.ctx);         // header + index; the device load follows once the shard is known
-        Region region, sregion;
-        const Region* rp = nullptr; const Region* srp = nullptr;
-        if (!o.region.empty()) { region = parse_region_arg(o.region, bam); rp = &region; }
-        if (!o.sample_region.empty()) { sregion = parse_region_arg(o.sample_region, bam); srp = &sregion; }
-        std::vector<RefTarget> targets;
-        for (uint32_t t = 0; t < bam.ref_names.size(); t++) {
-            if (rp) { if (bam.ref_names[t] == rp->name) targets.push_back({t, rp->start, rp->end - rp->start, rp->name}); }
-            else targets.push_back({t, 0, bam.ref_lens[t], bam.ref_names[t]});
-        }
-        IncludeBed include;
-        const IncludeBed* inc = nullptr;
-        if (!o.include_bed.empty()) {
-            std::map<std::string, uint32_t> name_to_tid;
-            for (auto& t : targets) name_to_tid[t.name] = t.tid;
-            include.read(o.include_bed, name_to_tid);
-            inc = &include;
-        }
-        bool combine_strands = o.combine_strands || o.hemi;        // pileup-hemi: the feeder runs in combine-strands mode
+        combine_strands = o.combine_strands || o.hemi;        // pileup-hemi: the feeder runs in combine-strands mode
         if (combine_strands && !(o.cpg || !o.motif_parts.empty())) throw std::runtime_error("need to specify either --motif or --cpg to combine strands");
-
-        mkp_params P;
-        memset(&P, 0, sizeof P);
         P.force_allow_implicit = o.force_allow;
         P.max_depth = o.max_depth;
         if (o.traditional) { P.numeric_mode = 2; P.collapse_code = 'h'; combine_strands = true; }
@@ -750,8 +747,6 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
         parse_edge_filter(o.edge, o.invert_edge, &P);
         // motifs (subcommand.rs:526-539, 592-612)
         std::vector<std::string> parts = o.motif_parts;
-        MotifContext mc;
-        bool have_motifs = false;
         if (o.hemi) { mc.motifs.push_back(hemi_m); have_motifs = true; }
         else if (!parts.empty()) {
             if (o.traditional) throw std::runtime_error("cannot use presets and motifs together");
@@ -764,493 +759,499 @@ inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* 
             for (size_t i = 0; i < parts.size(); i += 2) mc.motifs.push_back(parse_motif(parts[i], std::stoi(parts[i + 1])));
             have_motifs = true;
         } else if (o.traditional || o.cpg) { mc.motifs.push_back(parse_motif("CG", 0)); have_motifs = true; }
-        BedFormat fmt;
         fmt.mixed_delim = o.mixed;
         for (auto& m : mc.motifs) fmt.motif_labels.push_back(m.label());
         if (have_motifs) {
             if (o.ref_fp.empty()) throw std::runtime_error("reference fasta is required for using --motif or --cpg options");
             if (combine_strands) for (auto& m : mc.motifs) if (!m.palindromic) throw std::runtime_error("cannot combine strands with a motif that is not a palindrome");
-            mc.fasta.open(o.ref_fp);
             mc.keep_case = o.mask;
-            mc.include = inc;
             for (auto& m : mc.motifs) mc.longest = std::max<uint64_t>(mc.longest, m.len);
         }
-        // ---- reference intervals: boundaries now (cheap), focus positions of this rank's range in the background
+    }
+    // what the BAM header and the input files decide: the regions, the targets, --include-bed and the FASTA
+    void open_inputs(const PileupOptions& o, const BamReader& bam) {
+        if (!o.region.empty()) region = parse_region_arg(o.region, bam);
+        if (!o.sample_region.empty()) sregion = parse_region_arg(o.sample_region, bam);
+        for (uint32_t t = 0; t < bam.ref_names.size(); t++) {
+            if (region) { if (bam.ref_names[t] == region->name) targets.push_back({t, region->start, region->end - region->start, region->name}); }
+            else targets.push_back({t, 0, bam.ref_lens[t], bam.ref_names[t]});
+        }
+        if (!o.include_bed.empty()) {
+            std::map<std::string, uint32_t> name_to_tid;
+            for (auto& t : targets) name_to_tid[t.name] = t.tid;
+            include.read(o.include_bed, name_to_tid);
+            inc = &include;
+        }
+        if (have_motifs) { mc.fasta.open(o.ref_fp); mc.include = inc; }
+    }
+    // the reference intervals: boundaries and shard cuts now (cheap), the focus positions of this rank's range in the background
+    void lay_out(const PileupOptions& o, const BamReader& bam, const Collective& coll) {
+        iv_targets = inc ? targets_from_include_bed(*inc, targets, o.interval_size) : targets;
+        ivs = interval_grid(iv_targets, o.interval_size, combine_strands, have_motifs ? &mc : nullptr, &iv_owner);
+        my_i1 = ivs.size();
+        if (coll.world > 1) { const std::vector<size_t> cuts = shard_cuts(bam, ivs, coll.world); my_i0 = cuts[coll.rank]; my_i1 = cuts[coll.rank + 1]; }
+    }
+};
+
+// The records of the pileup: with the device ingest everything, or the byte ranges under this rank's intervals, is loaded on the
+// GPU. A BAM too big for it is read on the host: a front-end choice, not a compute fallback (the reads are sliced on the host and
+// uploaded chunk by chunk). That reader is one of its own, `host_bam`: the sampler may still be fetching through `bam`.
+inline BamReader& load_reads(const PileupOptions& o, const PileupPlan& plan, bool sharded, BamReader& bam, std::optional<BamReader>* host_bam) {
+    if (o.host_ingest) return bam;
+    if (!sharded) {
+        try { bam.load_default(); return bam; }
+        catch (const DeviceIngestTooBig& e) {
+            if (!o.quiet) fprintf(stderr, "> %s; reading the BAM on the host instead\n", e.what());
+            host_bam->emplace();
+            (*host_bam)->open(o.in_bam, o.threads);
+            return **host_bam;
+        }
+    }
+    std::vector<BamReader::Piece> pieces;
+    for (size_t i = plan.my_i0; i < plan.my_i1; i++) {
+        if (!pieces.empty() && pieces.back().tid == plan.ivs[i].tid) pieces.back().hi = std::max(pieces.back().hi, plan.ivs[i].end);
+        else pieces.push_back({plan.ivs[i].tid, plan.ivs[i].start, plan.ivs[i].end});
+    }
+    bam.load_pieces(pieces);
+    return bam;
+}
+
+// a chunk = consecutive intervals [c0, c1) of one contig, up to chunk_bp
+inline size_t chunk_end(const std::vector<RefInterval>& ivs, size_t c0, uint32_t chunk_bp) {
+    size_t c1 = c0 + 1;
+    while (c1 < ivs.size() && ivs[c1].tid == ivs[c0].tid && ivs[c1].start == ivs[c1 - 1].end && ivs[c1].end - ivs[c0].start <= chunk_bp) c1++;
+    return c1;
+}
+
+struct ChunkWork { size_t i0, i1; std::vector<RecRef> recs; };
+// The device work of the chunk [c0, c1) with reads `recs`. --max-depth (src/pileup/mod.rs:755-759 -> bam_plp_set_maxcnt): the
+// pileup engine of the reference runs per interval and drops reads while its buffer is full, so the reads that count can differ
+// from interval to interval. Only a chunk that holds more reads than the limit can be affected: it is then processed interval by
+// interval, each with the reads its own engine would keep. (Parity unpinned by the reference's tests; rule restated in
+// depth_limit_keep.)
+inline std::vector<ChunkWork> chunk_work(const std::vector<RefInterval>& ivs, size_t c0, size_t c1, std::vector<RecRef>&& recs, uint32_t max_depth) {
+    if (max_depth && recs.size() > max_depth) {
+        std::vector<ChunkWork> per_iv;
+        bool split = false;
+        for (size_t k = c0; k < c1; k++) {
+            ChunkWork w{k, k + 1, {}};
+            for (auto& r : recs) if (r.pos < (int64_t)ivs[k].end && r.end > (int64_t)ivs[k].start) w.recs.push_back(r);
+            const size_t before = w.recs.size();
+            depth_limit_keep(&w.recs, max_depth);
+            split = split || w.recs.size() != before;
+            per_iv.push_back(std::move(w));
+        }
+        if (split) return per_iv;
+    }
+    std::vector<ChunkWork> whole;
+    whole.push_back({c0, c1, std::move(recs)});
+    return whole;
+}
+
+// With --partition-tag one group of reads per key (each an independent pileup: src/pileup/mod.rs:795-830), in key order, "\1" for
+// the reads without a key; otherwise one group "" of all reads. Device-resident records give their tags on the GPU (mkp_bam_tags).
+inline std::map<std::string, std::vector<RecRef>> partition_groups(mkp_ctx* ctx, const BamReader& reads, const std::vector<std::string>& tags, std::vector<RecRef>&& recs) {
+    std::map<std::string, std::vector<RecRef>> groups;
+    if (tags.empty()) { groups[""] = std::move(recs); return groups; }
+    // only alignments the pileup admits create a key (flag filter of the pileup engine, pileup/mod.rs:783-791)
+    std::vector<RecRef> adm;
+    for (auto& r : recs) if (!((r.flag & (0x4 | 0x100 | 0x200 | 0x400 | 0x800)) || r.l_seq == 0)) adm.push_back(r);
+    std::vector<uint8_t> cells;
+    const size_t n_pt = tags.size();
+    if (reads.on_device && !adm.empty()) {
+        std::vector<uint32_t> ids(adm.size());
+        for (size_t k = 0; k < adm.size(); k++) ids[k] = adm[k].idx;
+        cells.resize(adm.size() * n_pt * MKP_TAG_CELL);
+        // four tags per call (mkp_bam_tags); the cells of a record are laid side by side in tag order
+        std::vector<uint8_t> part;
+        for (size_t t0 = 0; t0 < n_pt; t0 += 4) {
+            const size_t nt4 = std::min<size_t>(4, n_pt - t0);
+            std::string tg;
+            for (size_t t = t0; t < t0 + nt4; t++) tg += tags[t];
+            part.resize(adm.size() * nt4 * MKP_TAG_CELL);
+            check_mkp(ctx, mkp_bam_tags(ctx, ids.data(), (uint32_t)ids.size(), tg.c_str(), (uint32_t)nt4, part.data()));
+            for (size_t k = 0; k < adm.size(); k++)
+                memcpy(cells.data() + (k * n_pt + t0) * MKP_TAG_CELL, part.data() + k * nt4 * MKP_TAG_CELL, nt4 * MKP_TAG_CELL);
+        }
+    }
+    for (size_t k = 0; k < adm.size(); k++) {
+        std::string key;
+        const bool have = reads.on_device ? partition_key_of_cells(cells.data() + k * n_pt * MKP_TAG_CELL, n_pt, &key)
+                                          : partition_key_of(reads.rec(adm[k]), adm[k].size, tags, &key);
+        groups[have ? key : std::string("\1")].push_back(adm[k]);
+    }
+    return groups;
+}
+
+struct ChunkOut { size_t i0 = 0, i1 = 0; std::string key_name; std::vector<mkp_row> rows; std::vector<mkp_hemi_row> hemi_rows; bool last = false; };
+// From the device stage to the formatting stage: at most two finished chunks wait; row buffers travel back (no fresh pages per chunk)
+struct ChunkQueue {
+    std::mutex mu;
+    std::condition_variable cv;
+    std::deque<ChunkOut> q;
+    std::vector<std::vector<mkp_row>> spare_rows;
+    bool consumer_gone = false;
+    void push(ChunkOut&& co) { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return q.size() < 2 || consumer_gone; }); q.push_back(std::move(co)); cv.notify_all(); }
+    ChunkOut pop() { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return !q.empty(); }); ChunkOut co = std::move(q.front()); q.pop_front(); cv.notify_all(); return co; }
+    void take_spare(std::vector<mkp_row>* rows) { std::lock_guard<std::mutex> lk(mu); if (!spare_rows.empty()) { rows->swap(spare_rows.back()); spare_rows.pop_back(); } }
+    void recycle(std::vector<mkp_row>&& rows) { std::lock_guard<std::mutex> lk(mu); rows.clear(); if (spare_rows.size() < 4) spare_rows.push_back(std::move(rows)); }
+    void leave() { std::lock_guard<std::mutex> lk(mu); consumer_gone = true; cv.notify_all(); }
+};
+
+// One group of reads on the device: the chunk made resident (sliced on the GPU from device-resident records, or the packed reads
+// uploaded), the pass (pileup, or pileup-hemi over the intervals starting at `starts`), the rows copied into `co`
+inline void device_step(mkp_ctx* ctx, const BamReader& reads, const mkp_chunk& ch, bool hemi, const std::vector<uint32_t>& starts, int32_t hemi_partner,
+                        bool want_alg_bytes, PackedChunk* pc, ChunkOut* co, RunSummary* S) {
+    using clk = std::chrono::steady_clock;
+    const auto t0 = clk::now();
+    if (reads.on_device) device_chunk(reads, pc->recs, ch.start, ch.end, ch.focus_pos, ch.focus_neg);
+    else check_mkp(ctx, mkp_upload_chunk(ctx, &ch));
+    const auto t_s = clk::now();
+    mkp_stats st;
+    check_mkp(ctx, hemi ? mkp_hemi_resident(ctx, starts.data(), (uint32_t)starts.size(), hemi_partner, &st) : mkp_pileup_resident(ctx, &st));
+    const auto t_k = clk::now();
+    const mkp_row* rows = nullptr;
+    const mkp_hemi_row* hemi_rows = nullptr;
+    size_t n_rows = 0;
+    check_mkp(ctx, hemi ? mkp_fetch_hemi_rows(ctx, &hemi_rows, &n_rows) : mkp_fetch_rows(ctx, &rows, &n_rows));
+    S->slice_s += secs_between(t0, t_s); S->pass_s += secs_between(t_s, t_k); S->rowcopy_s += secs_between(t_k, clk::now());
+    if (want_alg_bytes && reads.on_device) {     // the headers of the reads the GPU sliced
+        pc->hdrs.resize(pc->recs.size());
+        uint32_t nr = 0;
+        check_mkp(ctx, mkp_fetch_chunk(ctx, pc->hdrs.data(), &nr, nullptr, nullptr));
+    }
+    if (hemi) co->hemi_rows.assign(hemi_rows, hemi_rows + n_rows);
+    else co->rows.assign(rows, rows + n_rows);          // the context's row buffer is reused by the next chunk
+    S->kernel_ms += st.kernel_ms[7];
+    S->algorithmic_bytes += (want_alg_bytes || !reads.on_device ? pc->algorithmic_bytes() : 0) + (hemi ? sizeof(mkp_hemi_row) : sizeof(mkp_row)) * n_rows;
+    S->reads_packed += pc->recs.size();
+    S->chunks++;
+    S->gpu_s += secs_between(t0, clk::now());
+}
+
+// The device stage: the reads of chunk after chunk, each unit of work and partition group through device_step, in output order
+inline void device_stage(mkp_ctx* ctx, const BamReader& reads, const PileupOptions& o, const PileupPlan& plan, ChunkQueue* queue, RunSummary* S) {
+    using clk = std::chrono::steady_clock;
+    const std::vector<RefInterval>& ivs = plan.ivs;
+    PackedChunk pc;
+    std::vector<uint32_t> fpos, fneg;
+    for (size_t c0 = 0, c1; c0 < ivs.size(); c0 = c1) {
+        c1 = chunk_end(ivs, c0, o.chunk_bp);
+        if (ivs[c1 - 1].end <= ivs[c0].start) continue;
+        std::vector<RecRef> recs;
+        reads.ensure_tid(ivs[c0].tid);
+        reads.for_overlapping(ivs[c0].tid, ivs[c0].start, ivs[c1 - 1].end, [&](const RecRef& r) { recs.push_back(r); });
+        if (recs.empty()) continue;
+        for (ChunkWork& wk : chunk_work(ivs, c0, c1, std::move(recs), o.max_depth)) {
+            const size_t i0 = wk.i0, i1 = wk.i1;
+            const uint32_t cs = ivs[i0].start, ce = ivs[i1 - 1].end;
+            if (ce <= cs || wk.recs.empty()) continue;
+            // pileup-hemi: the call window reaches the partner of every motif position; the reads stay those of the intervals
+            mkp_chunk ch{};
+            ch.start = cs - (plan.hemi_partner < 0 ? std::min<uint32_t>(cs, (uint32_t)-plan.hemi_partner) : 0);
+            ch.end = plan.hemi_partner > 0 ? (uint32_t)std::min<uint64_t>((uint64_t)ce + (uint32_t)plan.hemi_partner, std::max(ce, reads.ref_lens[ivs[i0].tid])) : ce;
+            std::vector<uint32_t> starts;
+            if (o.hemi) for (size_t k = i0; k < i1; k++) starts.push_back(ivs[k].start);
+            bool focus_done = false;
+            for (auto& grp : partition_groups(ctx, reads, o.partition_tags, std::move(wk.recs))) {
+                const auto ta = clk::now();
+                pc.clear();
+                if (reads.on_device) pc.recs = grp.second;
+                else pack_records_mt(reads, grp.second, o.threads, &pc);
+                if (pc.recs.empty()) continue;
+                ch.hdrs = pc.hdrs.data(); ch.n_reads = (uint32_t)pc.hdrs.size(); ch.heap = pc.heap.data(); ch.heap_bytes = pc.heap.size();
+                if (plan.have_motifs || plan.inc) { if (!focus_done) { focus_bitmaps(ivs, i0, i1, ch.start, ch.end, &fpos, &fneg); focus_done = true; } ch.focus_pos = fpos.data(); ch.focus_neg = fneg.data(); }
+                S->pack_s += secs_between(ta, clk::now());
+                ChunkOut co{i0, i1, grp.first == "\1" ? std::string("ungrouped") : grp.first};
+                queue->take_spare(&co.rows);
+                device_step(ctx, reads, ch, o.hemi, starts, plan.hemi_partner, !o.stats_json.empty(), &pc, &co, S);
+                queue->push(std::move(co));
+            }
+        }
+    }
+}
+
+// Where the text goes: a stream (stdout, or a file that is not regular); a regular file, which the formatting workers write in
+// place; a directory of files made on first use (--bedgraph / --partition-tag); or, in a sharded run, this rank's slice of the
+// one file, written at its offset at the end. The output is made first, like the reference, so a bad path fails before any work.
+class PileupWriter {
+    const std::string path_;
+    const Collective coll_;
+    FILE* out_ = nullptr;
+    int fd_ = -1;                      // out_ is a regular file: written in place, at pos_
+    uint64_t pos_ = 0;
+    std::map<std::string, FILE*> files_;
+    std::vector<std::string> parts_;                          // per formatting worker (capacity kept from chunk to chunk)
+    std::vector<std::map<std::string, std::string>> routed_;  // per formatting worker, to a directory: file name -> text
+    std::vector<std::string> slice_;   // sharded: the header (rank 0), then the formatted parts in order
+    static bool pwrite_all(int fd, const std::string& text, uint64_t offset) {
+        for (size_t done = 0; done < text.size();) {
+            const ssize_t w = pwrite(fd, text.data() + done, text.size() - done, (off_t)(offset + done));
+            if (w <= 0) return false;
+            done += (size_t)w;
+        }
+        return true;
+    }
+    FILE* file(const std::string& name) {
+        FILE*& f = files_[name];
+        if (!f && !(f = fopen((path_ + "/" + name).c_str(), "w"))) { files_.erase(name); throw std::runtime_error("failed to make output file " + path_ + "/" + name); }
+        return f;
+    }
+public:
+    PileupWriter(const PileupOptions& o, bool to_dir, const Collective& coll) : path_(o.out_bed), coll_(coll) {
+        if (coll.world > 1) {
+            if (coll.rank == 0) {
+                FILE* f = fopen(path_.c_str(), "w");     // created (and truncated) by rank 0 before the first exchange
+                if (!f) throw std::runtime_error("failed to make output file");
+                fclose(f);
+            }
+            slice_.push_back(coll.rank == 0 && o.header ? bed_header_line() : "");
+        } else if (!to_dir) {
+            out_ = (path_ == "-" || path_ == "stdout") ? stdout : fopen(path_.c_str(), "w");
+            if (!out_) throw std::runtime_error("failed to make output file");
+            if (o.header) fputs(bed_header_line(), out_);
+            if (out_ != stdout) {
+                fflush(out_);
+                struct stat sb;
+                const off_t at = ftello(out_);
+                if (at >= 0 && fstat(fileno(out_), &sb) == 0 && S_ISREG(sb.st_mode)) { fd_ = fileno(out_); pos_ = (uint64_t)at; }
+            }
+        } else {
+            std::error_code ec;
+            std::filesystem::create_directories(path_, ec);
+            if (ec) throw std::runtime_error("failed to create output directory " + path_);
+        }
+    }
+    ~PileupWriter() { if (out_ && out_ != stdout) fclose(out_); for (auto& kv : files_) fclose(kv.second); }
+
+    // one chunk, formatted by nt workers of the pool: format(t, text, files) fills worker t's text, or its files of a directory
+    void write_chunk(WorkerPool& pool, int nt, const std::function<void(int, std::string*, std::map<std::string, std::string>*)>& format) {
+        if ((int)parts_.size() < nt) { parts_.resize(nt); routed_.resize(nt); }
+        for (auto& p : parts_) p.clear();
+        for (auto& r : routed_) r.clear();
+        std::unique_ptr<std::atomic<uint64_t>[]> psize(new std::atomic<uint64_t>[nt]);
+        for (int t = 0; t < nt; t++) psize[t].store(UINT64_MAX);
+        std::atomic<bool> failed{false};
+        pool.run(nt, [&](int t) {
+            struct Publish { std::atomic<uint64_t>* a; ~Publish() { if (a->load() == UINT64_MAX) a->store(0); } } guard{&psize[t]};      // (a worker that leaves early must not block the others)
+            format(t, &parts_[t], &routed_[t]);
+            if (fd_ < 0) return;
+            // the text of worker t follows the text of the workers before it: wait for their sizes, then write in place
+            psize[t].store(parts_[t].size(), std::memory_order_release);
+            uint64_t at = pos_;
+            for (int q = 0; q < t; q++) { uint64_t v; while ((v = psize[q].load(std::memory_order_acquire)) == UINT64_MAX) std::this_thread::yield(); at += v; }
+            if (!pwrite_all(fd_, parts_[t], at)) failed = true;
+        });
+        if (failed) throw std::runtime_error("failed to write output file " + path_);
+        for (int t = 0; t < nt; t++) {
+            if (coll_.world > 1) { if (!parts_[t].empty()) slice_.push_back(std::move(parts_[t])); }
+            else if (fd_ >= 0) pos_ += parts_[t].size();
+            else if (out_) fwrite(parts_[t].data(), 1, parts_[t].size(), out_);
+            for (auto& kv : routed_[t]) if (!kv.second.empty()) fwrite(kv.second.data(), 1, kv.second.size(), file(kv.first));
+        }
+    }
+
+    // The end of the output. Sharded: rank-ordered concatenation (the reference's ordered collect, src/pileup/subcommand.rs:735-799):
+    // the slice sizes are exchanged (second and last collective) and every rank writes its slice at its offset, on the pool.
+    void finish(WorkerPool& pool, RunSummary* S) {
+        if (out_) { if (out_ != stdout) fclose(out_); else fflush(out_); out_ = nullptr; }
+        if (coll_.world <= 1) { S->rows_total = S->rows; S->positions_total = S->positions; return; }
+        const auto tw = std::chrono::steady_clock::now();
+        std::vector<uint64_t> sizes((size_t)coll_.world + 2, 0), at(slice_.size());
+        for (auto& s : slice_) sizes[coll_.rank] += s.size();
+        sizes[coll_.world] = S->rows; sizes[(size_t)coll_.world + 1] = S->positions;
+        coll_.sum(sizes.data(), sizes.size());
+        uint64_t a = std::accumulate(sizes.begin(), sizes.begin() + coll_.rank, (uint64_t)0);
+        for (size_t k = 0; k < slice_.size(); k++) { at[k] = a; a += slice_[k].size(); }
+        const int fd = ::open(path_.c_str(), O_WRONLY);
+        if (fd < 0) throw std::runtime_error("failed to open output file " + path_);
+        std::atomic<bool> failed{false};
+        pool.run((int)slice_.size(), [&](int k) { if (!failed && !pwrite_all(fd, slice_[k], at[k])) failed = true; });
+        ::close(fd);
+        if (failed) throw std::runtime_error("failed to write output file " + path_);
+        S->rows_total = sizes[coll_.world]; S->positions_total = sizes[(size_t)coll_.world + 1];
+        S->write_s += secs_between(tw, std::chrono::steady_clock::now());
+    }
+    void release_buffers() { parts_.clear(); parts_.shrink_to_fit(); slice_.clear(); slice_.shrink_to_fit(); }
+};
+
+// The rows of one chunk as text (position sorted: every interval gets its slice; intervals are formatted in parallel); row count
+inline uint64_t format_chunk(const ChunkOut& co, const PileupOptions& o, const PileupPlan& plan, const std::string& chrom, WorkerPool& pool, PileupWriter* out) {
+    const std::vector<RefInterval>& ivs = plan.ivs;
+    const size_t i0 = co.i0, n_iv = co.i1 - co.i0;
+    const mkp_row* rows = co.rows.data();
+    const size_t n_rows = o.hemi ? co.hemi_rows.size() : co.rows.size();
+    auto pos_of = [&](size_t j) { return o.hemi ? co.hemi_rows[j].pos : rows[j].pos; };
+    std::vector<size_t> rlo(n_iv + 1);
+    {
+        size_t r0 = 0;
+        for (size_t k = 0; k < n_iv; k++) { while (r0 < n_rows && pos_of(r0) < ivs[i0 + k].start) r0++; rlo[k] = r0; }
+        size_t r1 = rlo[n_iv - 1];
+        while (r1 < n_rows && pos_of(r1) < ivs[co.i1 - 1].end) r1++;
+        rlo[n_iv] = r1;
+    }
+    const int nt = std::max(1, std::min<int>(o.threads, (int)n_iv));
+    const std::string pfx = o.prefix.empty() ? std::string() : o.prefix + "_";
+    std::vector<uint64_t> part_rows(nt, 0);
+    out->write_chunk(pool, nt, [&](int t, std::string* text, std::map<std::string, std::string>* files) {
+        std::vector<OutRow> local;
+        for (size_t k = n_iv * t / nt; k < n_iv * (t + 1) / nt; k++) {
+            const size_t r_end = k + 1 < n_iv ? std::max(rlo[k], rlo[k + 1]) : rlo[n_iv];
+            size_t r1 = rlo[k];
+            while (r1 < r_end && pos_of(r1) < ivs[i0 + k].end) r1++;
+            if (o.hemi) {       // rows are final: one per (position, base, pattern), in output order
+                for (size_t j = rlo[k]; j < r1; j++) format_hemi_row(co.hemi_rows[j], chrom, o.mixed, text);
+                part_rows[t] += r1 - rlo[k];
+                continue;
+            }
+            local.clear();
+            finish_interval_rows(ivs[i0 + k], rows + rlo[k], r1 - rlo[k], plan.have_motifs ? &plan.mc.motifs : nullptr, plan.combine_strands, &local);
+            if (!plan.to_dir) for (auto& orow : local) format_bed_row(orow, chrom, plan.fmt, text);
+            else if (!o.bedgraph) { std::string& dst = (*files)[pfx + co.key_name + ".bed"]; for (auto& orow : local) format_bed_row(orow, chrom, plan.fmt, &dst); }
+            else for (auto& orow : local) {
+                std::string& dst = (*files)[pfx + co.key_name + (co.key_name.empty() ? "" : "_") + bedgraph_label(orow, plan.fmt) + "_" + strand_label(orow.strand) + ".bedgraph"];
+                format_bedgraph_row(orow, chrom, &dst);
+            }
+            part_rows[t] += local.size();
+        }
+    });
+    return std::accumulate(part_rows.begin(), part_rows.end(), (uint64_t)0);
+}
+
+inline int run_pileup(const PileupOptions& o, RunSummary* summary, std::string* error, const Collective* coll_in = nullptr) {
+    using clk = std::chrono::steady_clock;
+    const Collective coll = coll_in ? *coll_in : Collective();
+    const bool sharded = coll.world > 1;
+    try {
+        const auto t0 = clk::now();
+        trace_clock().epoch = t0;
+        auto trace = [&](const char* what) { trace_clock().mark(coll.rank, what); };
+        PileupPlan plan(o, sharded);
+        // the device comes first: with the device ingest (default) the BAM is inflated and sliced on the GPU
+        DeviceGuard dev{open_device(o.device)};
+        trace("device context created");
+        BamReader bam;
+        if (o.host_ingest) bam.open(o.in_bam, o.threads);
+        else bam.open_device_index(o.in_bam, dev.ctx);         // header + index; the device load follows once the shard is known
+        plan.open_inputs(o, bam);
         trace("index + fasta opened");
         const auto t_iv0 = clk::now();
-        std::vector<RefTarget> iv_targets = targets;
-        if (inc) iv_targets = targets_from_include_bed(*inc, iv_targets, o.interval_size);
-        std::vector<size_t> iv_owner;
-        std::vector<RefInterval> ivs = interval_grid(iv_targets, o.interval_size, combine_strands, have_motifs ? &mc : nullptr, &iv_owner);
-        size_t my_i0 = 0, my_i1 = ivs.size();
-        if (sharded) { const std::vector<size_t> cuts = shard_cuts(bam, ivs, coll.world); my_i0 = cuts[coll.rank]; my_i1 = cuts[coll.rank + 1]; }
+        plan.lay_out(o, bam, coll);
         // ---- threshold estimation. With the device ingest of an indexed BAM it starts now, beside the load: its candidates come
         // straight from the file (host fetch through the index), only its decode passes need the device and wait for `dev_ready`.
         // Otherwise it runs after the load, on the reads of the pileup.
         const bool estimate = o.filter_thresholds.empty() && !o.no_filtering;
         SamplerConfig sc;
-        SampleResult sample;
-        std::exception_ptr sample_err;
         std::shared_ptr<void> sample_garbage;
-        std::promise<void> dev_ready_p, sample_done_p;
-        std::shared_future<void> dev_ready_f = dev_ready_p.get_future().share();
-        std::future<void> sample_done_f = sample_done_p.get_future();
-        bool dev_ready_set = false;
+        std::promise<SampleResult> sample_p;
+        std::future<SampleResult> sample_f = sample_p.get_future();
         auto run_sampler = [&](const BamReader& src) {
-            try { sample = sample_histogram(src, dev.ctx, sc, coll); }
-            catch (...) { sample_err = std::current_exception(); }
-            sample_done_p.set_value();           // the result is out; the candidate buffers are released after that, beside the pileup
-            sample_garbage.reset();
+            try { sample_p.set_value(sample_histogram(src, dev.ctx, sc, coll)); }
+            catch (...) { sample_p.set_exception(std::current_exception()); }
+            sample_garbage.reset();              // the result is out; the candidate buffers are released after that, beside the pileup
         };
-        struct BgJoin { std::thread t; std::promise<void>* p; bool* set; ~BgJoin() { if (!*set) { try { p->set_value(); } catch (...) {} *set = true; } if (t.joinable()) t.join(); } } bg_job{std::thread(), &dev_ready_p, &dev_ready_set};
+        std::promise<void> dev_ready_p;
+        std::shared_future<void> dev_ready_f = dev_ready_p.get_future().share();
+        bool dev_ready_set = false;
+        auto set_dev_ready = [&]() { if (!dev_ready_set) { dev_ready_p.set_value(); dev_ready_set = true; } };
+        std::optional<BackgroundJob> sampler_job;
         trace("interval grid + shard cuts");
         if (estimate) {
             sc = sampler_config(o.schedule_threads > 0 ? o.schedule_threads : o.threads, o.sampling_interval_size, o.num_reads, o.have_frac, o.frac, false, "-n or -f 1.0");
             sc.workers = o.threads;
-            sc.region = srp ? srp : rp;
+            sc.region = plan.sregion ? &*plan.sregion : plan.region ? &*plan.region : nullptr;
             sc.include_unmapped = o.include_unmapped;
-            sc.edge_on = P.edge_filter_on;
-            sc.include = inc;
+            sc.edge_on = plan.P.edge_filter_on;
+            sc.include = plan.inc;
             sc.defer_free = &sample_garbage;
-            mkp_params PS = P;
+            mkp_params PS = plan.P;
             PS.max_depth = 0;           // the sampler looks at reads, not at pileup columns
-            if (mkp_set_params(dev.ctx, &PS)) throw std::runtime_error(mkp_last_error(dev.ctx));
-            if (!loaded && bam.have_index()) {
+            check_mkp(dev.ctx, mkp_set_params(dev.ctx, &PS));
+            if (!o.host_ingest && bam.have_index()) {
                 sc.device_ready = &dev_ready_f;
-                bg_job.t = std::thread(run_sampler, std::cref(bam));
+                sampler_job.emplace([&]() { run_sampler(bam); }, set_dev_ready);
             }
         }
-        // ---- focus positions of this rank's intervals (reference motif scan), beside the load and the sampler. Every object the
-        // job touches is declared above; its joiner is declared after them, so it is destroyed (joined) before they are.
-        std::exception_ptr iv_err;
+        // ---- focus positions of this rank's intervals (reference motif scan), beside the load and the sampler
         double iv_secs = 0;
-        struct Joiner { std::thread t; void join() { if (t.joinable()) t.join(); } ~Joiner() { join(); } } iv_job;
-        iv_job.t = std::thread([&]() {
-            try {
-                fill_interval_focus(ivs, my_i0, my_i1, iv_targets, iv_owner, combine_strands, have_motifs ? &mc : nullptr, inc, std::max(1, o.threads / 2));
-                iv_secs = secs(t_iv0, clk::now());
-                trace("interval focus filled (background)");
-            } catch (...) { iv_err = std::current_exception(); }
+        BackgroundJob iv_job([&]() {
+            fill_interval_focus(plan.ivs, plan.my_i0, plan.my_i1, plan.iv_targets, plan.iv_owner, plan.combine_strands, plan.have_motifs ? &plan.mc : nullptr, plan.inc, std::max(1, o.threads / 2));
+            iv_secs = secs_between(t_iv0, clk::now());
+            trace("interval focus filled (background)");
         });
-        // ---- device load: everything, or the byte ranges under this rank's intervals
         std::optional<BamReader> host_bam;
-        if (!loaded) {
-            if (sharded) {
-                std::vector<BamReader::Piece> pieces;
-                for (size_t i = my_i0; i < my_i1; i++) {
-                    if (!pieces.empty() && pieces.back().tid == ivs[i].tid) pieces.back().hi = std::max(pieces.back().hi, ivs[i].end);
-                    else pieces.push_back({ivs[i].tid, ivs[i].start, ivs[i].end});
-                }
-                bam.load_pieces(pieces);
-            } else {
-                try { bam.load_default(); }
-                catch (const DeviceIngestTooBig& e) {
-                    // a front-end choice, not a compute fallback: the reads are sliced on the host and uploaded chunk by chunk. A
-                    // reader of its own: the sampler may still be fetching through `bam`.
-                    if (!o.quiet) fprintf(stderr, "> %s; reading the BAM on the host instead\n", e.what());
-                    host_bam.emplace();
-                    host_bam->open(o.in_bam, o.threads);
-                }
-            }
-        }
-        BamReader& reads = host_bam ? *host_bam : bam;       // the records of the pileup
-        if (!dev_ready_set) { dev_ready_p.set_value(); dev_ready_set = true; }
+        BamReader& reads = load_reads(o, plan, sharded, bam, &host_bam);
+        set_dev_ready();
         const auto t_load = clk::now();
         trace("device load done");
         if (trace_clock().on) fprintf(stderr, "[mkh r%d]             ingest: h2d %.1f ms, inflate %.1f ms, record walk %.1f ms, total %.1f ms\n", coll.rank, reads.ingest_ms[0], reads.ingest_ms[1], reads.ingest_ms[2], reads.ingest_ms[3]);
         uint64_t any_mapped = 0;
-        for (auto& t : targets) if (rp || !inc || inc->has_contig(t.tid)) any_mapped += reads.stats.n_mapped[t.tid];
+        for (auto& t : plan.targets) if (plan.region || !plan.inc || plan.inc->has_contig(t.tid)) any_mapped += reads.stats.n_mapped[t.tid];
         if (!any_mapped) throw std::runtime_error("did not find any mapped reads, perform alignment first or use modkit extract and/or modkit summary to inspect unaligned modBAMs");
-        // output first, like the reference, so a bad path fails before any work
-        FILE* out = nullptr;
-        struct Router {          // files of the output directory, created on first use
-            std::string dir;
-            std::map<std::string, FILE*> files;
-            FILE* get(const std::string& name) {
-                auto it = files.find(name);
-                if (it != files.end()) return it->second;
-                FILE* f = fopen((dir + "/" + name).c_str(), "w");
-                if (!f) throw std::runtime_error("failed to make output file " + dir + "/" + name);
-                files[name] = f;
-                return f;
-            }
-            ~Router() { for (auto& kv : files) fclose(kv.second); }
-        } router;
-        std::string shard_text;      // sharded: this rank's slice of the output (header; the formatted parts follow in shard_parts), written at its offset at the end
-        std::vector<std::string> shard_parts;
-        int out_fd = -1;             // single regular output file: the formatting workers write their text at its offset (pwrite)
-        uint64_t file_pos = 0;
-        if (sharded) {
-            if (coll.rank == 0) {
-                FILE* f = fopen(o.out_bed.c_str(), "w");     // created (and truncated) by rank 0 before the first exchange
-                if (!f) throw std::runtime_error("failed to make output file");
-                fclose(f);
-                if (o.header) shard_text += bed_header_line();
-            }
-        } else if (!to_dir) {
-            out = (o.out_bed == "-" || o.out_bed == "stdout") ? stdout : fopen(o.out_bed.c_str(), "w");
-            if (!out) throw std::runtime_error("failed to make output file");
-            if (o.header) fputs(bed_header_line(), out);
-            if (out != stdout) {
-                fflush(out);
-                struct stat sb;
-                const off_t at = ftello(out);
-                if (at >= 0 && fstat(fileno(out), &sb) == 0 && S_ISREG(sb.st_mode)) { out_fd = fileno(out); file_pos = (uint64_t)at; }
-            }
-        } else {
-            std::error_code ec;
-            std::filesystem::create_directories(o.out_bed, ec);
-            if (ec) throw std::runtime_error("failed to create output directory " + o.out_bed);
-            router.dir = o.out_bed;
-        }
-        const std::string pfx = o.prefix.empty() ? std::string() : o.prefix + "_";
+        PileupWriter out(o, plan.to_dir, coll);
 
         // thresholds (subcommand.rs:615-638, command_utils.rs:49-134)
-        parse_mod_thresholds(o.mod_thresholds, &P);
-        parse_filter_thresholds(o.filter_thresholds, &P);
+        parse_mod_thresholds(o.mod_thresholds, &plan.P);
+        parse_filter_thresholds(o.filter_thresholds, &plan.P);
+        SampleResult sample;
         if (estimate) {
-            if (!bg_job.t.joinable()) run_sampler(reads);
-            sample_done_f.wait();
+            if (!sampler_job) run_sampler(reads);
+            sample_f.wait();
             trace("sampler result");
-            if (sample_err) std::rethrow_exception(sample_err);
-            estimated_thresholds(sample, o.percentile, "exact histogram quantile impossible; pass --filter-threshold", !o.quiet && coll.rank == 0, &P);
+            sample = sample_f.get();
+            estimated_thresholds(sample, o.percentile, "exact histogram quantile impossible; pass --filter-threshold", !o.quiet && coll.rank == 0, &plan.P);
         }
-        if (mkp_set_params(dev.ctx, &P)) throw std::runtime_error(mkp_last_error(dev.ctx));
-        if (summary) for (int b = 0; b < 4; b++) { summary->thresholds[b] = P.base_threshold[b]; summary->threshold_set[b] = P.base_threshold_set[b]; }
+        check_mkp(dev.ctx, mkp_set_params(dev.ctx, &plan.P));
         const auto t_thr = clk::now();
         trace("thresholds done");
 
         iv_job.join();
-        if (iv_err) std::rethrow_exception(iv_err);
-        const auto t_iv = clk::now();
-        (void)t_iv;
         RunSummary S;
         S.fetch_s = sample.fetch_s;
-        if (sharded) { ivs.erase(ivs.begin() + (ptrdiff_t)my_i1, ivs.end()); ivs.erase(ivs.begin(), ivs.begin() + (ptrdiff_t)my_i0); }
+        std::vector<RefInterval>& ivs = plan.ivs;
+        if (sharded) { ivs.erase(ivs.begin() + (ptrdiff_t)plan.my_i1, ivs.end()); ivs.erase(ivs.begin(), ivs.begin() + (ptrdiff_t)plan.my_i0); }
         for (auto& iv : ivs) S.positions += iv.end - iv.start;
 
         // ---- two stages: a device thread selects the reads of chunk after chunk, slices them on the GPU, runs the pass and takes
         // the rows; this thread turns finished chunks into text (strand combining, formatting: parallel over intervals) and
         // writes them in order. The device works on chunk k + 1 while chunk k is being formatted.
-        struct ChunkOut { size_t i0 = 0, i1 = 0; std::string key_name; std::vector<mkp_row> rows; std::vector<mkp_hemi_row> hemi_rows; bool last = false; };
-        std::mutex q_mu;
-        std::condition_variable q_cv;
-        std::deque<ChunkOut> queue;
-        std::vector<std::vector<mkp_row>> spare_rows;       // row buffers travel back to the device stage (no fresh pages per chunk)
-        std::exception_ptr dev_err;
-        bool consumer_gone = false;
-        const bool want_alg_bytes = !o.stats_json.empty();
-        auto push_out = [&](ChunkOut&& co) {
-            std::unique_lock<std::mutex> lk(q_mu);
-            q_cv.wait(lk, [&] { return queue.size() < 2 || consumer_gone; });
-            queue.push_back(std::move(co));
-            q_cv.notify_all();
-        };
-        auto device_stage = [&]() {
-            try {
-                PackedChunk pc;
-                std::vector<uint32_t> fpos, fneg;
-                for (size_t c0 = 0; c0 < ivs.size();) {
-                    // a chunk = consecutive intervals of one contig up to chunk_bp
-                    size_t c1 = c0 + 1;
-                    while (c1 < ivs.size() && ivs[c1].tid == ivs[c0].tid && ivs[c1].start == ivs[c1 - 1].end && ivs[c1].end - ivs[c0].start <= o.chunk_bp) c1++;
-                    if (ivs[c1 - 1].end <= ivs[c0].start) { c0 = c1; continue; }
-                    // the reads of the chunk
-                    std::vector<RecRef> chunk_recs;
-                    reads.ensure_tid(ivs[c0].tid);
-                    reads.for_overlapping(ivs[c0].tid, ivs[c0].start, ivs[c1 - 1].end, [&](const RecRef& r) { chunk_recs.push_back(r); });
-                    if (chunk_recs.empty()) { c0 = c1; continue; }
-                    // --max-depth (src/pileup/mod.rs:755-759 -> bam_plp_set_maxcnt): the pileup engine of the reference runs per interval
-                    // and drops reads while its buffer is full, so the reads that count can differ from interval to interval. Only a
-                    // chunk that holds more reads than the limit can be affected: it is then processed interval by interval, each with
-                    // the reads its own engine would keep. (Parity unpinned by the reference's tests; rule restated in depth_limit_keep.)
-                    struct Work { size_t a, b; std::vector<RecRef> recs; };
-                    std::vector<Work> work;
-                    bool split = false;
-                    if (o.max_depth && chunk_recs.size() > o.max_depth) {
-                        std::vector<Work> per_iv;
-                        for (size_t k = c0; k < c1; k++) {
-                            Work w{k, k + 1, {}};
-                            for (auto& r : chunk_recs) if (r.pos < (int64_t)ivs[k].end && r.end > (int64_t)ivs[k].start) w.recs.push_back(r);
-                            const size_t before = w.recs.size();
-                            depth_limit_keep(&w.recs, o.max_depth);
-                            split = split || w.recs.size() != before;
-                            per_iv.push_back(std::move(w));
-                        }
-                        if (split) work.swap(per_iv);
-                    }
-                    if (!split) { Work w{c0, c1, {}}; w.recs.swap(chunk_recs); work.push_back(std::move(w)); }
-                    for (auto& wk : work) {
-                        const size_t i0 = wk.a, i1 = wk.b;
-                        const uint32_t cs = ivs[i0].start, ce = ivs[i1 - 1].end;
-                        if (ce <= cs || wk.recs.empty()) continue;
-                        // pileup-hemi: the call window reaches the partner of every motif position; the reads stay those of the intervals
-                        uint32_t wcs = cs, wce = ce;
-                        if (hemi_partner < 0) wcs = cs - std::min<uint32_t>(cs, (uint32_t)-hemi_partner);
-                        if (hemi_partner > 0) wce = (uint32_t)std::min<uint64_t>((uint64_t)ce + (uint32_t)hemi_partner, std::max(ce, reads.ref_lens[ivs[i0].tid]));
-                        std::vector<RecRef>& all_recs = wk.recs;
-                        // with --partition-tag one group per key (each an independent pileup: src/pileup/mod.rs:795-830), in key order
-                        std::map<std::string, std::vector<RecRef>> groups;
-                        if (!partitioned) groups[""].swap(all_recs);
-                        else {
-                            // only alignments the pileup admits create a key (flag filter of the pileup engine, pileup/mod.rs:783-791)
-                            std::vector<RecRef> adm;
-                            for (auto& r : all_recs) if (!((r.flag & (0x4 | 0x100 | 0x200 | 0x400 | 0x800)) || r.l_seq == 0)) adm.push_back(r);
-                            std::vector<uint8_t> cells;
-                            const size_t n_pt = o.partition_tags.size();
-                            if (reads.on_device && !adm.empty()) {
-                                std::vector<uint32_t> ids(adm.size());
-                                for (size_t k = 0; k < adm.size(); k++) ids[k] = adm[k].idx;
-                                cells.resize(adm.size() * n_pt * MKP_TAG_CELL);
-                                // four tags per call (mkp_bam_tags); the cells of a record are laid side by side in tag order
-                                std::vector<uint8_t> part;
-                                for (size_t t0 = 0; t0 < n_pt; t0 += 4) {
-                                    const size_t nt4 = std::min<size_t>(4, n_pt - t0);
-                                    std::string tg;
-                                    for (size_t t = t0; t < t0 + nt4; t++) tg += o.partition_tags[t];
-                                    part.resize(adm.size() * nt4 * MKP_TAG_CELL);
-                                    if (mkp_bam_tags(dev.ctx, ids.data(), (uint32_t)ids.size(), tg.c_str(), (uint32_t)nt4, part.data())) throw std::runtime_error(mkp_last_error(dev.ctx));
-                                    for (size_t k = 0; k < adm.size(); k++)
-                                        memcpy(cells.data() + (k * n_pt + t0) * MKP_TAG_CELL, part.data() + k * nt4 * MKP_TAG_CELL, nt4 * MKP_TAG_CELL);
-                                }
-                            }
-                            for (size_t k = 0; k < adm.size(); k++) {
-                                std::string key;
-                                const bool have = reads.on_device ? partition_key_of_cells(cells.data() + k * n_pt * MKP_TAG_CELL, n_pt, &key)
-                                                                  : partition_key_of(reads.rec(adm[k]), adm[k].size, o.partition_tags, &key);
-                                groups[have ? key : std::string("\1")].push_back(adm[k]);
-                            }
-                        }
-                        bool focus_done = false;
-                        for (auto& grp : groups) {
-                            const auto ta = clk::now();
-                            pc.clear();
-                            if (reads.on_device) pc.recs = grp.second;
-                            else pack_records_mt(reads, grp.second, o.threads, &pc);
-                            if (pc.recs.empty()) continue;
-                            mkp_chunk ch;
-                            memset(&ch, 0, sizeof ch);
-                            ch.start = wcs; ch.end = wce; ch.hdrs = pc.hdrs.data(); ch.n_reads = (uint32_t)pc.hdrs.size(); ch.heap = pc.heap.data(); ch.heap_bytes = pc.heap.size();
-                            if (have_motifs || inc) { if (!focus_done) { focus_bitmaps(ivs, i0, i1, wcs, wce, &fpos, &fneg); focus_done = true; } ch.focus_pos = fpos.data(); ch.focus_neg = fneg.data(); }
-                            const auto tb = clk::now();
-                            S.pack_s += secs(ta, tb);
-                            const mkp_row* rows = nullptr;
-                            const mkp_hemi_row* hemi_rows = nullptr;
-                            size_t n_rows = 0;
-                            mkp_stats st;
-                            auto hemi_pass = [&]() {
-                                std::vector<uint32_t> starts;
-                                for (size_t k = i0; k < i1; k++) starts.push_back(ivs[k].start);
-                                if (mkp_hemi_resident(dev.ctx, starts.data(), (uint32_t)starts.size(), hemi_partner, &st)) throw std::runtime_error(mkp_last_error(dev.ctx));
-                            };
-                            if (reads.on_device) {
-                                // slice on the GPU (no packed chunk in host memory), then the same kernels
-                                device_chunk(reads, pc.recs, wcs, wce, ch.focus_pos, ch.focus_neg);
-                                const auto t_s = clk::now();
-                                S.slice_s += secs(tb, t_s);
-                                if (o.hemi) hemi_pass();
-                                else if (mkp_pileup_resident(dev.ctx, &st)) throw std::runtime_error(mkp_last_error(dev.ctx));
-                                const auto t_k = clk::now();
-                                S.pass_s += secs(t_s, t_k);
-                                if (o.hemi ? mkp_fetch_hemi_rows(dev.ctx, &hemi_rows, &n_rows) : mkp_fetch_rows(dev.ctx, &rows, &n_rows)) throw std::runtime_error(mkp_last_error(dev.ctx));
-                                S.rowcopy_s += secs(t_k, clk::now());
-                                if (want_alg_bytes) {
-                                    pc.hdrs.resize(pc.recs.size());
-                                    uint32_t nr = 0;
-                                    if (mkp_fetch_chunk(dev.ctx, pc.hdrs.data(), &nr, nullptr, nullptr)) throw std::runtime_error(mkp_last_error(dev.ctx));
-                                }
-                            } else if (o.hemi) {
-                                if (mkp_upload_chunk(dev.ctx, &ch)) throw std::runtime_error(mkp_last_error(dev.ctx));
-                                hemi_pass();
-                                if (mkp_fetch_hemi_rows(dev.ctx, &hemi_rows, &n_rows)) throw std::runtime_error(mkp_last_error(dev.ctx));
-                            } else if (mkp_pileup_chunk(dev.ctx, &ch, &rows, &n_rows, &st)) throw std::runtime_error(mkp_last_error(dev.ctx));
-                            ChunkOut co;
-                            co.i0 = i0; co.i1 = i1;
-                            co.key_name = !partitioned ? std::string() : (grp.first == "\1" ? std::string("ungrouped") : grp.first);
-                            { std::lock_guard<std::mutex> lk(q_mu); if (!spare_rows.empty()) { co.rows.swap(spare_rows.back()); spare_rows.pop_back(); } }
-                            if (o.hemi) co.hemi_rows.assign(hemi_rows, hemi_rows + n_rows);
-                            else co.rows.assign(rows, rows + n_rows);          // the context's row buffer is reused by the next chunk
-                            S.gpu_s += secs(tb, clk::now());
-                            S.kernel_ms += st.kernel_ms[7];
-                            S.reads_packed += pc.recs.size();
-                            S.algorithmic_bytes += (want_alg_bytes || !reads.on_device ? pc.algorithmic_bytes() : 0) + (o.hemi ? sizeof(mkp_hemi_row) : sizeof(mkp_row)) * n_rows;
-                            S.chunks++;
-                            push_out(std::move(co));
-                        }
-                    }
-                    c0 = c1;
-                }
-            } catch (...) { dev_err = std::current_exception(); }
-            trace("device stage done");
-            ChunkOut fin;
-            fin.last = true;
-            push_out(std::move(fin));
-        };
-        struct DevJoiner { std::thread t; std::mutex* mu; std::condition_variable* cv; bool* gone;
-                           ~DevJoiner() { { std::lock_guard<std::mutex> g(*mu); *gone = true; } cv->notify_all(); if (t.joinable()) t.join(); } } dev_job{std::thread(), &q_mu, &q_cv, &consumer_gone};
-        dev_job.t = std::thread(device_stage);
+        ChunkQueue queue;
+        BackgroundJob dev_job([&]() {
+            auto close_queue = [&]() { trace("device stage done"); ChunkOut fin; fin.last = true; queue.push(std::move(fin)); };
+            try { device_stage(dev.ctx, reads, o, plan, &queue, &S); }
+            catch (...) { close_queue(); throw; }
+            close_queue();
+        }, [&]() { queue.leave(); });
         WorkerPool pool(std::max(1, o.threads));
-        std::vector<std::string> part_pool;
-        for (;;) {
-            ChunkOut co;
-            {
-                std::unique_lock<std::mutex> lk(q_mu);
-                q_cv.wait(lk, [&] { return !queue.empty(); });
-                co = std::move(queue.front());
-                queue.pop_front();
-                q_cv.notify_all();
-            }
-            if (co.last) break;
+        for (ChunkOut co = queue.pop(); !co.last; co = queue.pop()) {
             const auto tc = clk::now();
-            const size_t i0 = co.i0, i1 = co.i1;
-            const mkp_row* rows = co.rows.data();
-            const size_t n_rows = o.hemi ? co.hemi_rows.size() : co.rows.size();
-            auto pos_of = [&](size_t j) { return o.hemi ? co.hemi_rows[j].pos : rows[j].pos; };
-            const std::string& key_name = co.key_name;
-            // rows are position sorted: every interval gets its slice; intervals are finished and formatted in parallel
-            const std::string& chrom = reads.ref_names[ivs[i0].tid];
-            const size_t n_iv = i1 - i0;
-            std::vector<size_t> rlo(n_iv + 1);
-            {
-                size_t r0 = 0;
-                for (size_t i = i0; i < i1; i++) { while (r0 < n_rows && pos_of(r0) < ivs[i].start) r0++; rlo[i - i0] = r0; }
-                size_t r1 = rlo[n_iv - 1];
-                while (r1 < n_rows && pos_of(r1) < ivs[i1 - 1].end) r1++;
-                rlo[n_iv] = r1;
-            }
-            const int nt = std::max(1, std::min<int>(o.threads, (int)n_iv));
-            std::vector<std::string>& parts = part_pool;
-            if ((int)parts.size() < nt) parts.resize(nt);
-            for (auto& ps : parts) ps.clear();                               // (capacity kept from the chunks before)
-            std::vector<std::map<std::string, std::string>> routed(nt);      // to_dir: file name -> text, per worker
-            std::vector<uint64_t> part_rows(nt, 0);
-            const bool direct = out_fd >= 0 && !to_dir && !sharded;
-            std::unique_ptr<std::atomic<uint64_t>[]> psize(new std::atomic<uint64_t>[nt]);
-            for (int t = 0; t < nt; t++) psize[t].store(UINT64_MAX);
-            std::atomic<bool> write_failed{false};
-            {
-                auto work = [&](int t) {
-                    struct Publish { std::atomic<uint64_t>* a; ~Publish() { if (a->load() == UINT64_MAX) a->store(0); } } guard{&psize[t]};      // (a worker that leaves early must not block the others)
-                    std::vector<OutRow> local;
-                    const size_t a = n_iv * t / nt, b = n_iv * (t + 1) / nt;
-                    for (size_t k = a; k < b; k++) {
-                        const size_t r_end = k + 1 < n_iv ? std::max(rlo[k], rlo[k + 1]) : rlo[n_iv];
-                        size_t r1 = rlo[k];
-                        while (r1 < r_end && pos_of(r1) < ivs[i0 + k].end) r1++;
-                        if (o.hemi) {       // rows are final: one per (position, base, pattern), in output order
-                            for (size_t j = rlo[k]; j < r1; j++) format_hemi_row(co.hemi_rows[j], chrom, o.mixed, &parts[t]);
-                            part_rows[t] += r1 - rlo[k];
-                            continue;
-                        }
-                        local.clear();
-                        finish_interval_rows(ivs[i0 + k], rows + rlo[k], r1 - rlo[k], have_motifs ? &mc.motifs : nullptr, combine_strands, &local);
-                        if (!to_dir) for (auto& orow : local) format_bed_row(orow, chrom, fmt, &parts[t]);
-                        else if (!o.bedgraph) { std::string& dst = routed[t][pfx + key_name + ".bed"]; for (auto& orow : local) format_bed_row(orow, chrom, fmt, &dst); }
-                        else for (auto& orow : local) {
-                            std::string label;
-                            std::string& dst = routed[t][pfx + key_name + (key_name.empty() ? "" : "_") + bedgraph_label(orow, fmt) + "_" + strand_label(orow.strand) + ".bedgraph"];
-                            format_bedgraph_row(orow, chrom, &dst);
-                        }
-                        part_rows[t] += local.size();
-                    }
-                    if (direct) {
-                        // the text of worker t follows the text of the workers before it: wait for their sizes, then write in place
-                        psize[t].store(parts[t].size(), std::memory_order_release);
-                        uint64_t at = file_pos;
-                        for (int q = 0; q < t; q++) { uint64_t v; while ((v = psize[q].load(std::memory_order_acquire)) == UINT64_MAX) std::this_thread::yield(); at += v; }
-                        size_t done = 0;
-                        while (done < parts[t].size()) {
-                            const ssize_t w = pwrite(out_fd, parts[t].data() + done, parts[t].size() - done, (off_t)(at + done));
-                            if (w <= 0) { write_failed = true; break; }
-                            done += (size_t)w;
-                        }
-                    }
-                };
-                pool.run(nt, work);
-            }
-            if (write_failed) throw std::runtime_error("failed to write output file " + o.out_bed);
-            for (int t = 0; t < nt; t++) {
-                if (sharded) { if (!parts[t].empty()) shard_parts.push_back(std::move(parts[t])); }
-                else if (direct) file_pos += parts[t].size();
-                else if (out) fwrite(parts[t].data(), 1, parts[t].size(), out);
-                for (auto& kv : routed[t]) if (!kv.second.empty()) fwrite(kv.second.data(), 1, kv.second.size(), router.get(kv.first));
-                S.rows += part_rows[t];
-            }
-            { std::lock_guard<std::mutex> lk(q_mu); co.rows.clear(); if (spare_rows.size() < 4) spare_rows.push_back(std::move(co.rows)); }
-            S.write_s += secs(tc, clk::now());
+            S.rows += format_chunk(co, o, plan, reads.ref_names[ivs[co.i0].tid], pool, &out);
+            queue.recycle(std::move(co.rows));
+            S.write_s += secs_between(tc, clk::now());
         }
         trace("last chunk formatted");
-        if (dev_job.t.joinable()) dev_job.t.join();
-        if (dev_err) std::rethrow_exception(dev_err);
-        if (out) { if (out != stdout) fclose(out); else fflush(out); }
-        if (sharded) {
-            // rank-ordered concatenation (the reference's ordered collect, src/pileup/subcommand.rs:735-799): the slice sizes
-            // are exchanged (second and last collective) and every rank writes its slice at its offset
-            const auto tw = clk::now();
-            std::vector<uint64_t> sizes((size_t)coll.world + 2, 0);
-            uint64_t my_bytes = shard_text.size();
-            for (auto& sp : shard_parts) my_bytes += sp.size();
-            sizes[coll.rank] = my_bytes;
-            sizes[coll.world] = S.rows; sizes[(size_t)coll.world + 1] = S.positions;
-            coll.sum(sizes.data(), sizes.size());
-            uint64_t at = 0;
-            for (int r = 0; r < coll.rank; r++) at += sizes[r];
-            const int fd = ::open(o.out_bed.c_str(), O_WRONLY);
-            if (fd < 0) throw std::runtime_error("failed to open output file " + o.out_bed);
-            // the pieces (header, then the formatted parts in order) go to their offsets from several threads
-            std::vector<std::pair<const std::string*, uint64_t>> pieces;
-            pieces.push_back({&shard_text, at});
-            { uint64_t q = at + shard_text.size(); for (auto& sp : shard_parts) { pieces.push_back({&sp, q}); q += sp.size(); } }
-            std::atomic<size_t> next_piece{0};
-            std::atomic<bool> failed{false};
-            auto put = [&]() {
-                for (;;) {
-                    const size_t k = next_piece.fetch_add(1);
-                    if (k >= pieces.size() || failed) break;
-                    const std::string& txt = *pieces[k].first;
-                    size_t done = 0;
-                    while (done < txt.size()) {
-                        const ssize_t w = pwrite(fd, txt.data() + done, txt.size() - done, (off_t)(pieces[k].second + done));
-                        if (w <= 0) { failed = true; break; }
-                        done += (size_t)w;
-                    }
-                }
-            };
-            {
-                std::vector<std::thread> th;
-                const int nw = (int)std::max<size_t>(1, std::min<size_t>((size_t)std::max(1, o.threads), pieces.size()));
-                for (int t = 1; t < nw; t++) th.emplace_back(put);
-                put();
-                for (auto& t : th) t.join();
-            }
-            ::close(fd);
-            if (failed) throw std::runtime_error("failed to write output file " + o.out_bed);
-            S.rows_total = sizes[coll.world]; S.positions_total = sizes[(size_t)coll.world + 1];
-            S.write_s += secs(tw, clk::now());
-        } else { S.rows_total = S.rows; S.positions_total = S.positions; }
+        dev_job.join();
+        out.finish(pool, &S);
         const auto t1 = clk::now();
         trace("output written");
-        S.load_s = secs(t0, t_load); S.threshold_s = secs(t_load, t_thr); S.interval_s = iv_secs;   /* runs beside ingest + thresholds; wait time = secs(t_thr, t_iv) */ S.total_s = secs(t0, t1);
-        for (int b = 0; b < 4; b++) { S.thresholds[b] = P.base_threshold[b]; S.threshold_set[b] = P.base_threshold_set[b]; }
+        S.load_s = secs_between(t0, t_load); S.threshold_s = secs_between(t_load, t_thr); S.interval_s = iv_secs;   /* runs beside ingest + thresholds */ S.total_s = secs_between(t0, t1);
+        for (int b = 0; b < 4; b++) { S.thresholds[b] = plan.P.base_threshold[b]; S.threshold_set[b] = plan.P.base_threshold_set[b]; }
         if (summary) *summary = S;
-        if (!o.quiet && (!sharded || coll.rank == 0))
+        if (!o.quiet && coll.rank == 0)
             fprintf(stderr, "> Done, processed %llu rows. positions=%llu reads=%llu chunks=%llu load=%.3fs thresholds=%.3fs intervals=%.3fs pack=%.3fs gpu=%.3fs (kernels %.3f ms) write=%.3fs total=%.3fs\n",
                     (unsigned long long)S.rows, (unsigned long long)S.positions, (unsigned long long)S.reads_packed, (unsigned long long)S.chunks,
                     S.load_s, S.threshold_s, S.interval_s, S.pack_s, S.gpu_s, S.kernel_ms, S.write_s, S.total_s);
-        if (!o.stats_json.empty()) {
-            FILE* jf = fopen(o.stats_json.c_str(), "w");
-            if (jf) {
-                fprintf(jf, "{\"positions\": %llu, \"rows\": %llu, \"reads\": %llu, \"chunks\": %llu, \"algorithmic_bytes\": %llu, \"load_s\": %.6f, \"thresholds_s\": %.6f, \"intervals_s\": %.6f, \"pack_s\": %.6f, \"gpu_s\": %.6f, \"kernel_ms\": %.6f, \"write_s\": %.6f, \"total_s\": %.6f, \"ingest\": \"%s\", \"ingest_h2d_ms\": %.3f, \"ingest_inflate_ms\": %.3f, \"ingest_walk_ms\": %.3f, \"sampler_fetch_s\": %.6f, \"slice_s\": %.6f, \"pass_s\": %.6f, \"rowcopy_s\": %.6f}\n",
-                        (unsigned long long)S.positions, (unsigned long long)S.rows, (unsigned long long)S.reads_packed, (unsigned long long)S.chunks, (unsigned long long)S.algorithmic_bytes,
-                        S.load_s, S.threshold_s, S.interval_s, S.pack_s, S.gpu_s, S.kernel_ms, S.write_s, S.total_s,
-                        reads.on_device ? (reads.ranged() ? "device-ranged" : "device") : "host", reads.ingest_ms[0], reads.ingest_ms[1], reads.ingest_ms[2], S.fetch_s, S.slice_s, S.pass_s, S.rowcopy_s);
-                fclose(jf);
-            }
+        if (FILE* jf = o.stats_json.empty() ? nullptr : fopen(o.stats_json.c_str(), "w")) {
+            fprintf(jf, "{\"positions\": %llu, \"rows\": %llu, \"reads\": %llu, \"chunks\": %llu, \"algorithmic_bytes\": %llu, \"load_s\": %.6f, \"thresholds_s\": %.6f, \"intervals_s\": %.6f, \"pack_s\": %.6f, \"gpu_s\": %.6f, \"kernel_ms\": %.6f, \"write_s\": %.6f, \"total_s\": %.6f, \"ingest\": \"%s\", \"ingest_h2d_ms\": %.3f, \"ingest_inflate_ms\": %.3f, \"ingest_walk_ms\": %.3f, \"sampler_fetch_s\": %.6f, \"slice_s\": %.6f, \"pass_s\": %.6f, \"rowcopy_s\": %.6f}\n",
+                    (unsigned long long)S.positions, (unsigned long long)S.rows, (unsigned long long)S.reads_packed, (unsigned long long)S.chunks, (unsigned long long)S.algorithmic_bytes,
+                    S.load_s, S.threshold_s, S.interval_s, S.pack_s, S.gpu_s, S.kernel_ms, S.write_s, S.total_s,
+                    reads.on_device ? (reads.ranged() ? "device-ranged" : "device") : "host", reads.ingest_ms[0], reads.ingest_ms[1], reads.ingest_ms[2], S.fetch_s, S.slice_s, S.pass_s, S.rowcopy_s);
+            fclose(jf);
         }
         if (trace_clock().on) {      // (development: where the release of the run's host objects goes)
             trace("stats written");
             std::vector<RefInterval>().swap(ivs); trace("intervals released");
-            part_pool.clear(); part_pool.shrink_to_fit(); shard_parts.clear(); shard_parts.shrink_to_fit(); spare_rows.clear(); spare_rows.shrink_to_fit(); trace("text + row buffers released");
+            out.release_buffers(); std::vector<std::vector<mkp_row>>().swap(queue.spare_rows); trace("text + row buffers released");
             reads.release_host_tables(); trace("record tables released");
         }
         return 0;
@@ -1456,8 +1457,7 @@ inline SampleResult sample_for_summary(const SampleOptions& o, mkp_ctx* ctx, boo
 
 inline int run_summary(const SampleOptions& o, std::string* text, std::string* error) {
     try {
-        DeviceGuard dev;
-        { const int rc = mkp_create(o.device, &dev.ctx); if (rc) throw std::runtime_error("no usable CUDA device (mkp_create returned " + std::to_string(rc) + "); this build has no CPU fallback"); }
+        DeviceGuard dev{open_device(o.device)};
         if (o.percentile > 1.0f) throw std::runtime_error("filter percentile must be <= 1.0");
         BamReader bam;
         mkp_params P;
@@ -1711,8 +1711,7 @@ inline void write_text_file(const std::filesystem::path& fp, const std::string& 
 inline int run_sample_probs(const SampleOptions& o, std::string* text, std::string* error) {
     try {
         const HistColors colors = check_sample_outputs(o);
-        DeviceGuard dev;
-        { const int rc = mkp_create(o.device, &dev.ctx); if (rc) throw std::runtime_error("no usable CUDA device (mkp_create returned " + std::to_string(rc) + "); this build has no CPU fallback"); }
+        DeviceGuard dev{open_device(o.device)};
         std::vector<float> qs;
         for (size_t i = 0; i < o.percentiles.size();) {
             size_t j = o.percentiles.find(',', i); if (j == std::string::npos) j = o.percentiles.size();
