@@ -254,6 +254,9 @@ int  mkp_bam_tags(mkp_ctx* ctx, const uint32_t* rec_ids, uint32_t n, const char*
  * (hdrs: n_reads entries or NULL; heap: *heap_bytes capacity in, bytes out; or NULL to query sizes). */
 int  mkp_bam_inflated(mkp_ctx* ctx, uint64_t off, uint8_t* dst, size_t len);
 int  mkp_fetch_chunk(mkp_ctx* ctx, mkp_read_hdr* hdrs, uint32_t* n_reads, uint8_t* heap, uint64_t* heap_bytes);
+/* Test access: the resident chunk's work items of the base-counting kernel, 5 words each {read, r_lo, first op, its query
+ * start, its reference start} (items: *n_items capacity in items, count out; or NULL to query the count). */
+int  mkp_fetch_count_items(mkp_ctx* ctx, uint32_t* items, uint32_t* n_items);
 
 /* SURVEY §8(d) algorithmic bytes of a chunk: sum over reads of 32 + 4 n_cigar + ceil(l_seq/2) + len_mm + len_ml,
  * plus 40 bytes per emitted row (roofline accounting only). */

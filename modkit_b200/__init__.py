@@ -58,7 +58,7 @@ HIST_BINS = 2049        # MKP_HIST_BINS (include/mkp.h): bins k/1024 of mkp_samp
 MKP_SYMBOLS = ["mkp_create", "mkp_bind_host_thread", "mkp_destroy", "mkp_last_error", "mkp_set_params", "mkp_upload_chunk", "mkp_pileup_resident",
                "mkp_fetch_rows", "mkp_pileup_chunk", "mkp_sample_histogram", "mkp_sample_histogram_wide", "mkp_sample_summary", "mkp_sample_mod_histogram", "mkp_algorithmic_bytes", "mkp_kernel_launches",
                "mkp_device_memory", "mkp_bam_load", "mkp_bam_load_range", "mkp_bam_load_range_fd", "mkp_bam_records", "mkp_bam_chunk", "mkp_bam_tags", "mkp_bam_inflated", "mkp_fetch_chunk",
-               "mkp_hemi_resident", "mkp_fetch_hemi_rows"]
+               "mkp_fetch_count_items", "mkp_hemi_resident", "mkp_fetch_hemi_rows"]
 MKH_SYMBOLS = ["mkh_pileup_main", "mkh_bam_open", "mkh_bam_close", "mkh_bam_n_refs", "mkh_bam_ref_name", "mkh_bam_ref_len",
                "mkh_bam_n_mapped", "mkh_bam_n_records", "mkh_pack_region", "mkh_packed_free", "mkh_packed_n_reads",
                "mkh_packed_hdrs", "mkh_packed_heap", "mkh_packed_heap_bytes", "mkh_packed_algorithmic_bytes", "mkh_format_rows",
@@ -125,6 +125,8 @@ def load_library(build_if_missing=True):
     lib.mkp_bam_tags.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_char_p, C.c_uint32, C.c_void_p]
     lib.mkp_bam_inflated.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_size_t]
     lib.mkp_fetch_chunk.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32), C.c_void_p, C.POINTER(C.c_uint64)]
+    if hasattr(lib, "mkp_fetch_count_items"):       # (older builds loaded as MODKIT_B200_LIB variants lack it)
+        lib.mkp_fetch_count_items.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32)]
     lib.mkh_bam_open_device.argtypes = [C.c_char_p, C.c_void_p, C.POINTER(C.c_void_p)]
     lib.mkh_device_chunk.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]
     lib.mkh_device_chunk.restype = C.c_int64
@@ -633,6 +635,15 @@ class Context:
         cap = C.c_uint64(hb.value)
         self._check(self._lib.mkp_fetch_chunk(self._h, hdrs.ctypes.data if n.value else None, C.byref(n), heap.ctypes.data if hb.value else None, C.byref(cap)))
         return hdrs, heap
+
+    def fetch_count_items(self):
+        """The resident chunk's work items of k_count_bases, as a (n, 5) uint32 array of {read, r_lo, op, q, r} (tests)."""
+        n = C.c_uint32()
+        self._check(self._lib.mkp_fetch_count_items(self._h, None, C.byref(n)))
+        items = np.zeros((n.value, 5), dtype=np.uint32)
+        if n.value:
+            self._check(self._lib.mkp_fetch_count_items(self._h, items.ctypes.data, C.byref(n)))
+        return items
 
     def close(self):
         if self._h:

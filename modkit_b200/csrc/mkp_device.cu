@@ -81,6 +81,9 @@ struct mkp_ctx {
     // focus-rank pass (chunks with focus bitmaps): tile table, rank of the focus set (built at upload), capacities
     DevBuf d_pscr, d_inftab, d_tiles, d_order;
     bool order_ready = false;
+    // work items of k_count_bases (CountItem, built at upload): items per read, their exclusive prefix (+ total), the table
+    DevBuf d_item_cnt, d_item_base, d_items;
+    uint32_t n_items = 0;
     uint32_t n_tiles = 0;
     bool tile_attr_set = false;
     uint32_t n_hot = 0, state_cap = 4, p_stride = 0;
@@ -117,9 +120,11 @@ struct PassScratch {
     uint32_t read_counter;                   // FusedDev::read_counter
     uint32_t tile_counter;                   // TileDev::tile_counter
     uint32_t tag_overflow;                   // k_tag_values
+    uint32_t n_items;                        // upload: work items of k_count_bases (scan total)
 };
 static_assert(sizeof(PassScratch) == 336 && offsetof(PassScratch, n_states) == 272 && offsetof(PassScratch, work) == 288 &&
-              offsetof(PassScratch, read_counter) == 320 && offsetof(PassScratch, tag_overflow) == 328, "d_small layout");
+              offsetof(PassScratch, read_counter) == 320 && offsetof(PassScratch, tag_overflow) == 328 && offsetof(PassScratch, n_items) == 332,
+              "d_small layout");
 
 static int fail(mkp_ctx* c, const std::string& m, int code = -1) { if (c) c->err = m; return code; }
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail(ctx, std::string(#call) + ": " + cudaGetErrorString(e_)); } while (0)
@@ -232,7 +237,7 @@ int mkp_upload_chunk(mkp_ctx* ctx, const mkp_chunk* ch) {
     if (!ctx || !ch) return -1;
     if (ch->end <= ch->start) return fail(ctx, "empty chunk range");
     CK(cudaSetDevice(ctx->device));
-    ctx->n_reads = ch->n_reads; ctx->cs = ch->start; ctx->ce = ch->end;
+    ctx->n_reads = ch->n_reads; ctx->cs = ch->start; ctx->ce = ch->end; ctx->n_items = 0;
     ctx->n_words = (ch->end - ch->start + 31) / 32;
     ctx->heap_bytes = ch->heap_bytes;
     ctx->h_entry_off.resize((size_t)ch->n_reads + 1);
@@ -386,6 +391,7 @@ static CountDev count_dev(const mkp_ctx* ctx, const ChunkDev& C, uint32_t stride
     D.obs_word = ctx->d_obs_word.as<uint32_t>(); D.work = C.work + 2;
     D.list = nullptr; D.list_count = nullptr;
     D.order = nullptr;          // (the counting kernels keep the coordinate order: neighbouring reads update neighbouring slots)
+    D.items = ctx->d_items.as<CountItem>(); D.n_items = ctx->n_items;
     return D;
 }
 
@@ -397,7 +403,7 @@ static int count_side_by_side(mkp_ctx* ctx, const CountDev& D) {
     CK(cudaStreamWaitEvent(ctx->stream2, ctx->ev_fork, 0));
     launch(ctx, k_count_calls, g2, 256, 0, ctx->stream2, D);
     CK(cudaEventRecord(ctx->ev_join, ctx->stream2));
-    launch(ctx, k_count_bases, g2, 256, 0, ctx->stream, D);
+    launch(ctx, k_count_bases, std::max(1, std::min(ctx->sm_count * 8, (int)((D.n_items + 7) / 8))), 256, 0, ctx->stream, D);
     CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
     return 0;
 }
@@ -429,10 +435,47 @@ static void pass_ms(const mkp_ctx* ctx, bool ranked, float* ms) {
 
 // Chunks with focus bitmaps: the positions that can produce rows are known at upload, so the rank structure (counter slot of
 // every focus position) and the tile table of k_pileup_tile are built here, once per chunk, not once per pass.
+// The work items of k_count_bases (CountItem): one per window of MKP_COUNT_ITEM_BP reference bases (default COUNT_ITEM_BP) of
+// every read that overlaps the chunk, built on the device in two steps around the host sync that ends the upload: the items per
+// read and their scan (the total lands in the scratch block), then the fill into a table of that size.
+constexpr uint32_t COUNT_ITEM_BP = 32768;
+static int count_items(mkp_ctx* ctx, uint32_t* S_out) {
+    uint32_t S = COUNT_ITEM_BP;
+    if (const char* e = getenv("MKP_COUNT_ITEM_BP")) {
+        const unsigned long v = strtoul(e, nullptr, 10);
+        if (v == 0 || v % 32 || v > 0x40000000ul) return fail(ctx, "MKP_COUNT_ITEM_BP must be a multiple of 32 between 32 and 2^30");
+        S = (uint32_t)v;
+    }
+    *S_out = S;
+    const uint32_t n = ctx->n_reads;
+    CK(ctx->d_small.ensure(sizeof(PassScratch)));
+    CK(ctx->d_item_cnt.ensure((size_t)std::max<uint32_t>(n, 1) * 4));
+    CK(ctx->d_item_base.ensure((size_t)n * 4 + 4));
+    uint32_t* const cnt = ctx->d_item_cnt.as<uint32_t>();
+    uint32_t* const total = &ctx->d_small.as<PassScratch>()->n_items;
+    if (!n) { CK(cudaMemsetAsync(total, 0, 4, ctx->stream)); return 0; }
+    launch(ctx, k_items_count, (n + 7) / 8, 256, 0, ctx->stream, ctx->d_hdrs.as<mkp_read_hdr>(), ctx->d_heap.as<uint8_t>(), n, ctx->cs, ctx->ce, S, cnt);
+    uint32_t* const base = ctx->d_item_base.as<uint32_t>();
+    if (int rc = exclusive_scan_u32(ctx, cnt, n, base, base + n)) return rc;        // (base[n]: the end of the last read's items)
+    CK(cudaMemcpyAsync(total, base + n, 4, cudaMemcpyDeviceToDevice, ctx->stream));
+    return 0;
+}
+static int fill_items(mkp_ctx* ctx, uint32_t S, uint32_t n_items) {
+    const uint32_t n = ctx->n_reads;
+    CK(ctx->d_items.ensure(std::max<size_t>(1, n_items) * sizeof(CountItem)));
+    ctx->n_items = n_items;
+    if (n_items)
+        launch(ctx, k_items_fill, (n + 7) / 8, 256, 0, ctx->stream, ctx->d_hdrs.as<mkp_read_hdr>(), ctx->d_heap.as<uint8_t>(), n, ctx->cs, S,
+               ctx->d_item_base.as<uint32_t>(), ctx->d_items.as<CountItem>());
+    return 0;
+}
+
 static int finish_upload(mkp_ctx* ctx) {
     ctx->focus_ready = false;
     ctx->order_ready = false;
     cudaStream_t st = ctx->stream;
+    uint32_t item_bp = 0;
+    if (int rc = count_items(ctx, &item_bp)) return rc;
     if (ctx->n_reads >= 4096 && !getenv("MKP_NO_ORDER")) {            // processing order of the read queues: longest reads first
         CK(ctx->d_order.ensure((size_t)ctx->n_reads * 4 + 32 * 4));
         uint32_t* hist = ctx->d_order.as<uint32_t>() + ctx->n_reads;
@@ -443,7 +486,11 @@ static int finish_upload(mkp_ctx* ctx) {
         launch(ctx, k_order_scatter, g, 256, 0, st, ctx->d_hdrs.as<mkp_read_hdr>(), ctx->n_reads, hist, ctx->d_order.as<uint32_t>());
         ctx->order_ready = true;
     }
-    if (!ctx->have_focus) { CK(cudaStreamSynchronize(st)); CK(cudaGetLastError()); return 0; }
+    if (!ctx->have_focus) {
+        PassScratch h;
+        if (int rc = read_scratch(ctx, &h)) return rc;
+        return fill_items(ctx, item_bp, h.n_items);
+    }
     // counter slot of every (focus position, strand): its rank in the [2][n_words] pair (focus_pos, focus_neg)
     const uint32_t n_words = ctx->n_words;
     CK(ctx->d_hot.ensure((size_t)n_words * 8 + 4));
@@ -465,7 +512,7 @@ static int finish_upload(mkp_ctx* ctx) {
     if (int rc = read_scratch(ctx, &h)) return rc;
     ctx->n_hot = h.n_hot;
     ctx->focus_ready = true;
-    return 0;
+    return fill_items(ctx, item_bp, h.n_items);
 }
 
 // The focus-rank pass, for chunks with focus bitmaps: the counter slots are the rank built at upload, so everything is enqueued
@@ -1061,7 +1108,7 @@ int mkp_bam_chunk(mkp_ctx* ctx, uint32_t start, uint32_t end, const uint32_t* re
     auto now = [] { return std::chrono::steady_clock::now(); };
     auto since = [&](std::chrono::steady_clock::time_point t) { return std::chrono::duration<double>(now() - t).count(); };
     auto t0 = now();
-    ctx->n_reads = n; ctx->cs = start; ctx->ce = end;
+    ctx->n_reads = n; ctx->cs = start; ctx->ce = end; ctx->n_items = 0;
     ctx->n_words = (end - start + 31) / 32;
     CK(ctx->d_hdrs.ensure(std::max<size_t>(1, n) * sizeof(mkp_read_hdr)));
     CK(ctx->d_entry_off.ensure(((size_t)n + 1) * 8));
@@ -1147,6 +1194,18 @@ int mkp_fetch_chunk(mkp_ctx* ctx, mkp_read_hdr* hdrs, uint32_t* n_reads, uint8_t
 
 uint64_t mkp_kernel_launches(const mkp_ctx* ctx) { return ctx ? ctx->launches : 0; }
 
+int mkp_fetch_count_items(mkp_ctx* ctx, uint32_t* items, uint32_t* n_items) {
+    if (!ctx || !n_items) return -1;
+    CK(cudaSetDevice(ctx->device));
+    if (items) {
+        if (*n_items < ctx->n_items) return fail(ctx, "item buffer too small");
+        CK(cudaStreamSynchronize(ctx->stream));           // (the fill kernel of the upload may still run)
+        if (ctx->n_items) CK(cudaMemcpy(items, ctx->d_items.p, (size_t)ctx->n_items * sizeof(CountItem), cudaMemcpyDeviceToHost));
+    }
+    *n_items = ctx->n_items;
+    return 0;
+}
+
 size_t mkp_algorithmic_bytes(const mkp_chunk* ch, size_t n_rows) {
     size_t b = 0;
     for (uint32_t i = 0; i < ch->n_reads; i++) {
@@ -1165,6 +1224,28 @@ int mkp_debug_parse_clocks(unsigned long long* out, int n, int reset) {
     for (int k = 0; k < n && k < PCLK_N; k++) out[k] = v[k];
     if (reset) { memset(v, 0, sizeof v); if (cudaMemcpyToSymbol(g_parse_clk, v, sizeof v) != cudaSuccess) return -1; }
     return PCLK_N;
+}
+#endif
+
+#ifdef MKP_COUNT_CLOCKS
+// Measurement builds only: the k_count_bases item log (mkp_kernels.cuh, g_count_clk) of the current device. out == nullptr:
+// (re)arm a zeroed log of n records; else copy the first n records (32 bytes each) of the log to out. Returns 0.
+int mkp_debug_count_clocks(void* out, uint32_t n) {
+    static void* d_log = nullptr;
+    static uint32_t cap = 0;
+    if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+    if (!out) {
+        if (n > cap) {
+            if (d_log) cudaFree(d_log);
+            if (cudaMalloc(&d_log, (size_t)n * sizeof(CountClk)) != cudaSuccess) { d_log = nullptr; cap = 0; return -1; }
+            cap = n;
+            if (cudaMemcpyToSymbol(g_count_clk, &d_log, sizeof d_log) != cudaSuccess) return -1;
+        }
+        if (cudaMemset(d_log, 0, (size_t)cap * sizeof(CountClk)) != cudaSuccess) return -1;
+        return cudaMemcpyToSymbol(g_count_clk_cap, &cap, sizeof cap) == cudaSuccess ? 0 : -1;
+    }
+    if (n > cap) return -1;
+    return cudaMemcpy(out, d_log, (size_t)n * sizeof(CountClk), cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -1;
 }
 #endif
 

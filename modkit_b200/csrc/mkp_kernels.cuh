@@ -397,7 +397,8 @@ __device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t* P, uint32_t 
 #ifndef MKP_MINB_RESOLVE
 #define MKP_MINB_RESOLVE 7
 #endif
-// k_count_bases: 5 blocks of 256 threads = 48 registers, which leaves 12 bytes of spills. At 8 blocks (32 registers) its hot loop
+// k_count_bases: 5 blocks of 256 threads = 48 registers, which leaves 32 bytes of spills (8 before it took work items; the launch
+// bounds were not swept again). At 8 blocks (32 registers) its hot loop
 // spilled 128 / 152 bytes and the kernel took 1.41x as long on an H100 (profiles/README.md); 4 blocks (64 registers, no spills) is
 // slower than 5: the walk is latency bound and wants the warps
 #ifndef MKP_MINB_BASES
@@ -1678,6 +1679,64 @@ __device__ __forceinline__ uint32_t wslot(const uint4& r, uint32_t t, uint32_t b
     return (t == 0 ? r.z : r.w) + __popc(bm & ((1u << bit) - 1u));
 }
 
+// One work item of k_count_bases: the part [r_lo, r_hi) of a read's reference span inside the chunk, where r_hi is the next
+// item's r_lo when that item belongs to the same read, else the chunk end. op is the first CIGAR op whose reference end is past
+// r_lo, q and r its query and reference start. A read gets one item per window of S reference bases (k_items_count), and the
+// seams between its items lie on the chunk's 32-position word grid, so no bitmap word is split between two items.
+struct CountItem { uint32_t read, r_lo, op, q, r; };
+
+// items of a read whose span clipped to the chunk is [cs + a, cs + b), a < b: one if it is at most S long, else one per S
+// bases from the word that holds its start (the seams: cs + (a & ~31) + j * S, j >= 1)
+__host__ __device__ __forceinline__ uint32_t count_items_of(uint32_t a, uint32_t b, uint32_t S) {
+    return b - a <= S ? 1u : (b - 1u - (a & ~31u)) / S + 1u;
+}
+
+// warp per read: the read's reference span clipped to [cs, ce) and the number of its items (0 when it misses the chunk)
+__global__ void __launch_bounds__(256) k_items_count(const mkp_read_hdr* __restrict__ hdrs, const uint8_t* __restrict__ heap, uint32_t n_reads,
+                                                     uint32_t cs, uint32_t ce, uint32_t S, uint32_t* __restrict__ n_items) {
+    const uint32_t ri = blockIdx.x * 8 + (threadIdx.x >> 5), lane = lane_id();
+    if (ri >= n_reads) return;
+    const mkp_read_hdr h = hdrs[ri];
+    const uint32_t* cig = (const uint32_t*)(heap + h.off);
+    uint32_t rc = (uint32_t)h.ref_start;
+    for (uint32_t b0 = 0; b0 < h.n_cigar && rc < ce; b0 += 32) {      // (the part past the chunk end is not needed)
+        const uint32_t i = b0 + lane, c = i < h.n_cigar ? cig[i] : 0, op = c & 15;
+        rc += __reduce_add_sync(FULL, (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) ? c >> 4 : 0u);
+    }
+    const uint32_t lo = (uint32_t)h.ref_start > cs ? (uint32_t)h.ref_start : cs, hi = rc < ce ? rc : ce;
+    if (lane == 0) n_items[ri] = lo < hi ? count_items_of(lo - cs, hi - cs, S) : 0u;
+}
+
+// warp per read: the read's items at base[ri] ..; the lane whose op holds a seam writes that item
+__global__ void __launch_bounds__(256) k_items_fill(const mkp_read_hdr* __restrict__ hdrs, const uint8_t* __restrict__ heap, uint32_t n_reads,
+                                                    uint32_t cs, uint32_t S, const uint32_t* __restrict__ base, CountItem* __restrict__ items) {
+    const uint32_t ri = blockIdx.x * 8 + (threadIdx.x >> 5), lane = lane_id();
+    if (ri >= n_reads) return;
+    const uint32_t n = base[ri + 1] - base[ri];
+    if (!n) return;
+    const mkp_read_hdr h = hdrs[ri];
+    const uint32_t* cig = (const uint32_t*)(heap + h.off);
+    const uint32_t lo = (uint32_t)h.ref_start > cs ? (uint32_t)h.ref_start : cs, a0 = (lo - cs) & ~31u;
+    const uint32_t last = n == 1 ? lo : cs + a0 + (n - 1) * S;           // the last seam
+    CountItem* out = items + base[ri];
+    uint32_t qc = 0, rc = (uint32_t)h.ref_start;
+    for (uint32_t b0 = 0; b0 < h.n_cigar && rc <= last; b0 += 32) {
+        const uint32_t i = b0 + lane, c = i < h.n_cigar ? cig[i] : 0, op = c & 15, len = c >> 4;
+        const uint32_t ql = (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) ? len : 0;
+        const uint32_t rl = (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) ? len : 0;
+        const uint32_t qi = warp_incl_scan(ql), rr = warp_incl_scan(rl);
+        const uint32_t q0 = qc + qi - ql, r0 = rc + rr - rl, e = r0 + rl;
+        qc += __shfl_sync(FULL, qi, 31);
+        rc += __shfl_sync(FULL, rr, 31);
+        for (uint32_t j = r0 <= lo ? 0u : (r0 - cs - a0 + S - 1u) / S; rl && j < n; j++) {   // the seams in [r0, e)
+            const uint32_t s = j ? cs + a0 + j * S : lo;
+            if (s >= e) break;
+            CountItem it; it.read = ri; it.r_lo = s; it.op = i; it.q = q0; it.r = r0;
+            out[j] = it;
+        }
+    }
+}
+
 struct CountDev {
     const mkp_read_hdr* hdrs;
     const uint8_t* heap;
@@ -1690,11 +1749,33 @@ struct CountDev {
     uint32_t n_states;
     uint32_t n_words;
     uint32_t* obs_word;   // [2][n_words] observed-code masks of fully covered bitmap words
-    uint32_t* work;       // dynamic read counter
+    uint32_t* work;       // dynamic read / item counter
     const uint32_t* list; // list mode: the reads to count (k_pileup_fused counted the others) and their number
     const uint32_t* list_count;
-    const uint32_t* order; // else: processing order (longest reads first), or null
+    const uint32_t* order; // else (k_count_calls): processing order (longest reads first), or null
+    const CountItem* items;   // else (k_count_bases): the chunk's work items, in coordinate order
+    uint32_t n_items;
 };
+
+// MKP_COUNT_CLOCKS=1 (measurement builds only): k_count_bases logs every work item it takes from the queue into
+// g_count_clk[queue index] (when below g_count_clk_cap): the SM, %globaltimer at dequeue and at the warp's next dequeue, the read
+// and [r_lo, r_hi). %globaltimer, not clock64(): SM clocks are not comparable across SMs. Read back by mkp_debug_count_clocks.
+#ifdef MKP_COUNT_CLOCKS
+struct CountClk { unsigned long long t0, t1; uint32_t sm, read, r_lo, r_hi; };
+__device__ CountClk* g_count_clk;
+__device__ uint32_t g_count_clk_cap;
+__device__ __forceinline__ unsigned long long global_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
+// (the pending record lives in shared memory, so the measured kernel keeps the register budget of the default build)
+#define CCLK_INIT __shared__ CountClk s_cclk[8]; __shared__ uint32_t s_cclk_i[8]; if (lane == 0) s_cclk_i[wib] = 0xffffffffu
+#define CCLK_DEQ(ii) do { if (lane == 0) { const unsigned long long t_ = global_ns(); const uint32_t p_ = s_cclk_i[wib]; \
+    if (p_ < g_count_clk_cap) { s_cclk[wib].t1 = t_; g_count_clk[p_] = s_cclk[wib]; } \
+    uint32_t sm_; asm volatile("mov.u32 %0, %%smid;" : "=r"(sm_)); s_cclk[wib].t0 = t_; s_cclk[wib].sm = sm_; s_cclk_i[wib] = (ii); } } while (0)
+#define CCLK_ITEM(ri, lo, hi) do { if (lane == 0) { s_cclk[wib].read = (ri); s_cclk[wib].r_lo = (lo); s_cclk[wib].r_hi = (hi); } } while (0)
+#else
+#define CCLK_INIT do {} while (0)
+#define CCLK_DEQ(ii) do {} while (0)
+#define CCLK_ITEM(ri, lo, hi) do {} while (0)
+#endif
 
 // FeatureVector::add_feature + Tally::add_feature (src/pileup/mod.rs:176-193, 238-281) as counter updates, on reference strand t
 // at bit `bit` of the word with record r
@@ -1743,24 +1824,46 @@ __global__ void __launch_bounds__(256) k_count_calls(CountDev D) {
     }
 }
 
-// warp per read: every aligned base / deleted position that lands on a hot position, plus the observed-code
-// coverage of the read (src/pileup/mod.rs:831-835: unioned for every alignment at the position, deletions included,
-// reference skips excluded).  Coverage is recorded per 32-position bitmap word when the read covers the whole word
-// (one coalesced check-then-OR per word) and per hot position only in the partial words at the ends of a run.
+// warp per work item (the part [r_lo, r_hi) of a read, CountItem; one item per read in list mode): every aligned base / deleted
+// position that lands on a hot position, plus the observed-code coverage of the read (src/pileup/mod.rs:831-835: unioned for every
+// alignment at the position, deletions included, reference skips excluded).  Coverage is recorded per 32-position bitmap word when
+// the read covers the whole word (one coalesced check-then-OR per word) and per hot position only in the partial words at the ends
+// of a run. The items keep coordinate order, so that neighbouring warps update neighbouring counter slots, and a long read is
+// several items, so that it does not form the kernel's tail when it is dequeued late.
 __global__ void __launch_bounds__(256, MKP_MINB_BASES) k_count_bases(CountDev D) {
     __shared__ uint32_t s_op[8][32], s_q[8][32], s_r[8][33];   // the current batch of 32 ops: op|len<<4, query start, reference start
     __shared__ uint32_t s_mask[8][32];                          // positions of the current 32 words where this read has a call
+    __shared__ uint32_t s_lim[8][2];                            // the item's [r_lo, r_hi) (kept out of the walk's registers)
     const uint32_t lane = lane_id();
     const uint32_t wib = threadIdx.x >> 5;
+    CCLK_INIT;
     for (;;) {
-        uint32_t ri = 0;
-        if (lane == 0) { ri = atomicAdd(D.work, 1u); if (D.list) ri = ri < *D.list_count ? D.list[ri] : 0xffffffffu; else if (D.order && ri < D.n_reads) ri = D.order[ri]; }
-        ri = __shfl_sync(FULL, ri, 0);
-        if (ri >= D.n_reads) break;
+        uint32_t ii = 0;
+        if (lane == 0) ii = atomicAdd(D.work, 1u);
+        ii = __shfl_sync(FULL, ii, 0);
+        CCLK_DEQ(ii);
+        uint32_t ri, r_lo, r_hi;
+        CountItem it;
+        if (D.list) {
+            ri = ii < *D.list_count ? D.list[ii] : 0xffffffffu;
+            if (ri >= D.n_reads) break;
+            r_lo = 0; r_hi = D.ce;                              // (r_lo, the op and its start are the read's, below)
+        } else {
+            if (ii >= D.n_items) break;
+            it = D.items[ii];
+            ri = it.read; r_lo = it.r_lo;
+            r_hi = D.ce;
+            if (ii + 1 < D.n_items) { const CountItem nx = D.items[ii + 1]; if (nx.read == ri) r_hi = nx.r_lo; }
+        }
         const ReadMeta m = D.meta[ri];
         if (!(m.flags & 1)) continue;
         const mkp_read_hdr h = D.hdrs[ri];
         if ((uint32_t)m.ref_end <= D.cs || (uint32_t)h.ref_start >= D.ce) continue;
+        const uint32_t lo_read = (uint32_t)h.ref_start > D.cs ? (uint32_t)h.ref_start : D.cs;
+        if (D.list) { r_lo = lo_read; it.op = 0; it.q = 0; it.r = (uint32_t)h.ref_start; }
+        CCLK_ITEM(ri, r_lo, r_hi);
+        __syncwarp();
+        if (lane == 0) { s_lim[wib][0] = r_lo; s_lim[wib][1] = r_hi; }
         const uint32_t a = (h.flags & 0x10) ? 1u : 0u;
         const uint32_t* cig = (const uint32_t*)(D.heap + h.off);
         const uint8_t* seq = D.heap + h.off + 4ull * h.n_cigar;
@@ -1769,12 +1872,17 @@ __global__ void __launch_bounds__(256, MKP_MINB_BASES) k_count_bases(CountDev D)
         const uint32_t pm = has_mods ? m.pos_mask : 0u, nm = has_mods ? m.neg_mask : 0u;
         const bool merge = has_mods && (m.flags & 4) && m.n_calls > 0;
         const uint2* rcalls = D.calls + m.entry_off;
-        uint32_t cp = 0;                                        // call records consumed so far (ascending position)
-        // observed-code coverage of one run [ra, rb) of reference positions
+        // call records consumed so far (ascending position): on a later item of the read, the first record at or after r_lo
+        uint32_t cp = 0;
+        if (merge && r_lo > lo_read) {
+            uint32_t hi_k = m.n_calls;
+            while (cp < hi_k) { const uint32_t mid = (cp + hi_k) >> 1; if (rcalls[a ? m.n_calls - 1u - mid : mid].x < r_lo) cp = mid + 1; else hi_k = mid; }
+        }
+        // observed-code coverage of one run [ra, rb) of reference positions, inside the item
         auto cover = [&](uint32_t ra, uint32_t rb) {
             if (!(pm | nm)) return;
-            if (ra < D.cs) ra = D.cs;
-            if (rb > D.ce) rb = D.ce;
+            if (ra < s_lim[wib][0]) ra = s_lim[wib][0];
+            if (rb > s_lim[wib][1]) rb = s_lim[wib][1];
             if (ra >= rb) return;
             const uint32_t wl = (ra - D.cs + 31) >> 5, wh = (rb - D.cs) >> 5;   // words [wl, wh) are fully covered
             for (uint32_t w = wl + lane; w < wh; w += 32) {
@@ -1797,9 +1905,9 @@ __global__ void __launch_bounds__(256, MKP_MINB_BASES) k_count_bases(CountDev D)
             if (wl > wh) partial(ra, rb);                       // the run starts and ends inside one word
             else { partial(ra, D.cs + (wl << 5)); partial(D.cs + (wh << 5), rb); }
         };
-        uint32_t qc = 0, rc = (uint32_t)h.ref_start;
+        uint32_t qc = it.q, rc = it.r;
         uint32_t run_start = rc;                                // start of the current run without reference skips
-        for (uint32_t b0 = 0; b0 < h.n_cigar; b0 += 32) {
+        for (uint32_t b0 = it.op; b0 < h.n_cigar; b0 += 32) {
             uint32_t i = b0 + lane;
             uint32_t c = i < h.n_cigar ? cig[i] : 0;
             uint32_t op = c & 15, len = c >> 4;
@@ -1825,7 +1933,8 @@ __global__ void __launch_bounds__(256, MKP_MINB_BASES) k_count_bases(CountDev D)
             s_op[wib][lane] = op | (len << 4); s_q[wib][lane] = q0; s_r[wib][lane] = r0;
             if (lane == 0) s_r[wib][32] = R1;
             __syncwarp();
-            const uint32_t blo = R0 > D.cs ? R0 : D.cs, bhi = R1 < D.ce ? R1 : D.ce;
+            const uint32_t r_lo_ = s_lim[wib][0], r_hi_ = s_lim[wib][1];
+            const uint32_t blo = R0 > r_lo_ ? R0 : r_lo_, bhi = R1 < r_hi_ ? R1 : r_hi_;
             if (blo < bhi) {
                 const uint32_t w_first = (blo - D.cs) >> 5, w_last = (bhi - 1 - D.cs) >> 5;
                 for (uint32_t wt = w_first; wt <= w_last; wt += 32) {
@@ -1909,6 +2018,7 @@ __global__ void __launch_bounds__(256, MKP_MINB_BASES) k_count_bases(CountDev D)
                 }
             }
             __syncwarp();
+            if (rc >= s_lim[wib][1]) break;                     // the rest of the read is the next item's
         }
         cover(run_start, rc);
     }
