@@ -250,6 +250,12 @@ int  mkp_bam_chunk(mkp_ctx* ctx, uint32_t start, uint32_t end, const uint32_t* r
  * A text longer than MKP_TAG_CELL - 3 bytes is an error. */
 #define MKP_TAG_CELL 256
 int  mkp_bam_tags(mkp_ctx* ctx, const uint32_t* rec_ids, uint32_t n, const char* tags, uint32_t n_tags, uint8_t* out);
+/* The same values without a length limit. Per item k = i * n_tags + t: types[k] the aux type character (0 = absent or a B array),
+ * lens[k] the value length, offs[k] its offset in `values` (exclusive scan of lens); types / lens / offs hold n * n_tags entries.
+ * *total gets the bytes of all values. `values` (capacity `cap` bytes) is filled only when it holds *total bytes; otherwise, or
+ * with values = NULL, the call only sizes: call again with a buffer of *total bytes. More than 4 GiB of values in one call is an error. */
+int  mkp_bam_tag_values(mkp_ctx* ctx, const uint32_t* rec_ids, uint32_t n, const char* tags, uint32_t n_tags,
+                        uint8_t* types, uint32_t* lens, uint32_t* offs, uint8_t* values, uint64_t cap, uint64_t* total);
 /* Test / debug access: bytes of the inflated stream; headers and heap of the resident chunk
  * (hdrs: n_reads entries or NULL; heap: *heap_bytes capacity in, bytes out; or NULL to query sizes). */
 int  mkp_bam_inflated(mkp_ctx* ctx, uint64_t off, uint8_t* dst, size_t len);

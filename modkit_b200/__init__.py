@@ -57,7 +57,7 @@ HIST_BINS = 2049        # MKP_HIST_BINS (include/mkp.h): bins k/1024 of mkp_samp
 
 MKP_SYMBOLS = ["mkp_create", "mkp_bind_host_thread", "mkp_destroy", "mkp_last_error", "mkp_set_params", "mkp_upload_chunk", "mkp_pileup_resident",
                "mkp_fetch_rows", "mkp_pileup_chunk", "mkp_sample_histogram", "mkp_sample_histogram_wide", "mkp_sample_summary", "mkp_sample_mod_histogram", "mkp_algorithmic_bytes", "mkp_kernel_launches",
-               "mkp_device_memory", "mkp_bam_load", "mkp_bam_load_range", "mkp_bam_load_range_fd", "mkp_bam_records", "mkp_bam_chunk", "mkp_bam_tags", "mkp_bam_inflated", "mkp_fetch_chunk",
+               "mkp_device_memory", "mkp_bam_load", "mkp_bam_load_range", "mkp_bam_load_range_fd", "mkp_bam_records", "mkp_bam_chunk", "mkp_bam_tags", "mkp_bam_tag_values", "mkp_bam_inflated", "mkp_fetch_chunk",
                "mkp_fetch_count_items", "mkp_hemi_resident", "mkp_fetch_hemi_rows"]
 MKH_SYMBOLS = ["mkh_pileup_main", "mkh_bam_open", "mkh_bam_close", "mkh_bam_n_refs", "mkh_bam_ref_name", "mkh_bam_ref_len",
                "mkh_bam_n_mapped", "mkh_bam_n_records", "mkh_pack_region", "mkh_packed_free", "mkh_packed_n_reads",
@@ -65,7 +65,7 @@ MKH_SYMBOLS = ["mkh_pileup_main", "mkh_bam_open", "mkh_bam_close", "mkh_bam_n_re
                "mkh_motif_focus", "mkh_bam_open_device", "mkh_device_chunk", "mkh_bam_ingest_ms", "mkh_bam_total_records",
                "mkh_f32_display", "mkh_bam_partition_key", "mkh_bam_n_ranges", "mkh_pileup_main_sharded", "mkh_shard_plan",
                "mkh_bam_open_device_pieces", "mkh_bam_fetch", "mkh_summary_main", "mkh_sample_probs_main", "mkh_partition_key_of_cells", "mkh_bam_index_n_mapped", "mkh_pct2",
-               "mkh_pileup_hemi_main", "mkh_pileup_hemi_main_sharded", "mkh_probabilities_tsv"]
+               "mkh_pileup_hemi_main", "mkh_pileup_hemi_main_sharded", "mkh_probabilities_tsv", "mkh_agree_file_slices"]
 
 ALLREDUCE_FN = C.CFUNCTYPE(C.c_int, C.POINTER(C.c_uint64), C.c_size_t, C.c_void_p)
 
@@ -123,6 +123,11 @@ def load_library(build_if_missing=True):
     lib.mkp_bam_records.argtypes = [C.c_void_p, C.c_void_p]
     lib.mkp_bam_chunk.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     lib.mkp_bam_tags.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_char_p, C.c_uint32, C.c_void_p]
+    lib.mkp_bam_tag_values.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_char_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
+    lib.mkh_agree_file_slices.argtypes = [C.c_int, C.c_int, ALLREDUCE_FN, C.c_void_p, C.c_char_p, C.c_void_p, C.c_uint32,
+                                          C.c_char_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64]
+    lib.mkh_agree_file_slices.restype = C.c_int64
     lib.mkp_bam_inflated.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_size_t]
     lib.mkp_fetch_chunk.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32), C.c_void_p, C.POINTER(C.c_uint64)]
     if hasattr(lib, "mkp_fetch_count_items"):       # (older builds loaded as MODKIT_B200_LIB variants lack it)
@@ -232,6 +237,25 @@ def pileup_main_sharded(args, rank, world, allreduce, hemi=False):
     keys = ["total_s", "load_s", "thresholds_s", "gpu_s", "write_s", "rows_total", "positions_total", "rows_rank",
             "threshold_A", "threshold_C", "threshold_G", "threshold_T", "sampler_fetch_s", "intervals_s", "pack_s", "kernel_ms", "slice_s", "pass_s", "rowcopy_s"]
     return rc, dict(zip(keys, [float(x) for x in st]))
+
+
+def agree_file_slices(sizes, rank, world, allreduce):
+    """One rank's side of the file agreement of a sharded --partition-tag run: `sizes` maps this rank's file names to its byte
+    counts; `allreduce` as in pileup_main_sharded (None when world == 1). Every rank must call it. Returns
+    {name: (offset of this rank, total size)} over the union of the names."""
+    lib = load_library()
+    names = list(sizes)
+    blob = b"".join(n.encode() + b"\0" for n in names)
+    sz = np.array([sizes[n] for n in names], dtype=np.uint64)
+    cb = ALLREDUCE_FN(allreduce) if allreduce is not None else C.cast(None, ALLREDUCE_FN)
+    cap = 1 << 16                 # (the union is returned in one call: a second call would be a second exchange)
+    out_names = C.create_string_buffer(1 << 24)
+    off, tot = np.zeros(cap, dtype=np.uint64), np.zeros(cap, dtype=np.uint64)
+    n = lib.mkh_agree_file_slices(rank, world, cb, None, blob, sz.ctypes.data, len(names), out_names, len(out_names), off.ctypes.data, tot.ctypes.data, cap)
+    if n < 0 or n > cap:
+        raise MkpError("file agreement failed (%d)" % n)
+    got = out_names.raw.split(b"\0")[:n]
+    return {g.decode(): (int(off[k]), int(tot[k])) for k, g in enumerate(got)}
 
 
 def bam_fetch(bam_path, tid, beg, end):
@@ -348,8 +372,11 @@ class Bam:
 
     def partition_key(self, tid, i, tags):
         """--partition-tag key of the i-th record of contig tid (host-opened BAM): the key string, or None for NoKey."""
-        buf = C.create_string_buffer(4096)
-        rc = self._lib.mkh_bam_partition_key(self._h, tid, i, ":".join(tags).encode(), buf, 4096)
+        for cap in (4096, 1 << 24):          # (tag values have no length limit: a key that does not fit is asked again)
+            buf = C.create_string_buffer(cap)
+            rc = self._lib.mkh_bam_partition_key(self._h, tid, i, ":".join(tags).encode(), buf, cap)
+            if rc >= 0:
+                break
         if rc < 0:
             raise MkpError("partition key failed")
         return buf.value.decode() if rc == 1 else None
@@ -624,6 +651,19 @@ class Context:
                 raise RuntimeError("partition key too long")
             out.append(buf.value.decode() if rc == 1 else None)
         return out
+
+    def bam_tag_values(self, rec_ids, tags):
+        """Raw mkp_bam_tag_values of device-resident records for up to four tags: (types, lens, offs, values) with types / lens /
+        offs of shape (n, n_tags) (type 0: absent or a B array; a value is values[offs:offs + lens]) and values a byte string."""
+        ids = np.ascontiguousarray(rec_ids, dtype=np.uint32)
+        m = (len(ids), len(tags))
+        types, lens, offs = np.zeros(m, dtype=np.uint8), np.zeros(m, dtype=np.uint32), np.zeros(m, dtype=np.uint32)
+        total = C.c_uint64(0)
+        args = (self._h, ids.ctypes.data, len(ids), "".join(tags).encode(), len(tags), types.ctypes.data, lens.ctypes.data, offs.ctypes.data)
+        self._check(self._lib.mkp_bam_tag_values(*args, None, 0, C.byref(total)))
+        values = np.zeros(max(1, total.value), dtype=np.uint8)
+        self._check(self._lib.mkp_bam_tag_values(*args, values.ctypes.data, total.value, C.byref(total)))
+        return types, lens, offs, values[:total.value].tobytes()
 
     def fetch_chunk(self):
         """(headers, heap) of the resident chunk, copied back from the device (tests)."""

@@ -825,31 +825,31 @@ inline std::string f32_display(float v) {
     return std::string(buf, r.ptr);
 }
 
-// --partition-tag: get_stringable_aux (src/util.rs:670-688) + parse_tags_from_record (src/pileup/mod.rs:629-646):
-// tag values joined by '_', "missing" for absent ones; false when none of the tags is present (PartitionKey::NoKey)
-inline bool partition_key_of(const uint8_t* r, uint32_t size, const std::vector<std::string>& tags, std::string* key) {
-    const uint32_t l_name = r[8], n_cigar = load_le<uint16_t>(r + 12);
-    const uint32_t l_seq = (uint32_t)std::max(0, load_le<int32_t>(r + 16));
-    const uint8_t* aux = r + 32 + l_name + 4ull * n_cigar + (l_seq + 1) / 2 + l_seq;
-    const uint8_t* end = r + size;
+// --partition-tag: get_stringable_aux (src/util.rs:670-688): the text of one aux value of type `ty` at p (n: the length of a Z/H
+// text); false for a type that is not stringable (B arrays)
+inline bool aux_value_text(char ty, const uint8_t* p, size_t n, std::string* v) {
+    switch (ty) {
+        case 'Z': case 'H': v->assign((const char*)p, n); return true;
+        case 'A': v->assign(1, (char)p[0]); return true;
+        case 'c': *v = std::to_string((int)(int8_t)p[0]); return true;
+        case 'C': *v = std::to_string((unsigned)p[0]); return true;
+        case 's': *v = std::to_string(load_le<int16_t>(p)); return true;
+        case 'S': *v = std::to_string(load_le<uint16_t>(p)); return true;
+        case 'i': *v = std::to_string(load_le<int32_t>(p)); return true;
+        case 'I': *v = std::to_string(load_le<uint32_t>(p)); return true;
+        case 'f': *v = f32_display(load_le<float>(p)); return true;
+        default: return false;
+    }
+}
+
+// parse_tags_from_record (src/pileup/mod.rs:629-646): the values of tags 0 .. n_tags joined by '_', "missing" for absent ones;
+// false when none of the tags is present (PartitionKey::NoKey). value(i, &v) is the text of tag i, or false when it is absent.
+template <class Value>
+inline bool partition_key_join(size_t n_tags, Value&& value, std::string* key) {
     bool any = false;
-    std::string k;
-    for (size_t i = 0; i < tags.size(); i++) {
-        AuxHit h;
-        std::string v;
-        bool have = aux < end && aux_find(aux, end, tags[i][0], tags[i][1], &h);
-        if (have) switch (h.type) {
-            case 'Z': case 'H': v.assign((const char*)h.p, h.n); break;
-            case 'A': v.assign(1, (char)h.p[0]); break;
-            case 'c': v = std::to_string((int)(int8_t)h.p[0]); break;
-            case 'C': v = std::to_string((unsigned)h.p[0]); break;
-            case 's': v = std::to_string(load_le<int16_t>(h.p)); break;
-            case 'S': v = std::to_string(load_le<uint16_t>(h.p)); break;
-            case 'i': v = std::to_string(load_le<int32_t>(h.p)); break;
-            case 'I': v = std::to_string(load_le<uint32_t>(h.p)); break;
-            case 'f': v = f32_display(load_le<float>(h.p)); break;
-            default: have = false;
-        }
+    std::string k, v;
+    for (size_t i = 0; i < n_tags; i++) {
+        const bool have = value(i, &v);
         any = any || have;
         if (i) k += "_";
         k += have ? v : std::string("missing");
@@ -858,34 +858,31 @@ inline bool partition_key_of(const uint8_t* r, uint32_t size, const std::vector<
     return any;
 }
 
+// the key of a record read on the host
+inline bool partition_key_of(const uint8_t* r, uint32_t size, const std::vector<std::string>& tags, std::string* key) {
+    const uint32_t l_name = r[8], n_cigar = load_le<uint16_t>(r + 12);
+    const uint32_t l_seq = (uint32_t)std::max(0, load_le<int32_t>(r + 16));
+    const uint8_t* aux = r + 32 + l_name + 4ull * n_cigar + (l_seq + 1) / 2 + l_seq;
+    const uint8_t* end = r + size;
+    return partition_key_join(tags.size(), [&](size_t i, std::string* v) {
+        AuxHit h;
+        return aux < end && aux_find(aux, end, tags[i][0], tags[i][1], &h) && aux_value_text(h.type, h.p, h.n, v);
+    }, key);
+}
+
 // the same key from the MKP_TAG_CELL-byte (type, length, value) cells of mkp_bam_tags (device front end)
 inline bool partition_key_of_cells(const uint8_t* cells, size_t n_tags, std::string* key) {
-    bool any = false;
-    std::string k;
-    for (size_t i = 0; i < n_tags; i++) {
+    return partition_key_join(n_tags, [&](size_t i, std::string* v) {
         const uint8_t* c = cells + (size_t)MKP_TAG_CELL * i;
-        const char ty = (char)c[0];
-        const uint8_t* p = c + 2;
-        std::string v;
-        bool have = ty != 0;
-        if (have) switch (ty) {
-            case 'Z': case 'H': v.assign((const char*)p, c[1]); break;
-            case 'A': v.assign(1, (char)p[0]); break;
-            case 'c': v = std::to_string((int)(int8_t)p[0]); break;
-            case 'C': v = std::to_string((unsigned)p[0]); break;
-            case 's': v = std::to_string(load_le<int16_t>(p)); break;
-            case 'S': v = std::to_string(load_le<uint16_t>(p)); break;
-            case 'i': v = std::to_string(load_le<int32_t>(p)); break;
-            case 'I': v = std::to_string(load_le<uint32_t>(p)); break;
-            case 'f': v = f32_display(load_le<float>(p)); break;
-            default: have = false;
-        }
-        any = any || have;
-        if (i) k += "_";
-        k += have ? v : std::string("missing");
-    }
-    if (any) *key = k;
-    return any;
+        return c[0] != 0 && aux_value_text((char)c[0], c + 2, c[1], v);
+    }, key);
+}
+
+// the same key from the (type, length, offset) items of mkp_bam_tag_values (device front end, values of any length)
+inline bool partition_key_of_values(const uint8_t* types, const uint32_t* lens, const uint64_t* offs, const uint8_t* values, size_t n_tags, std::string* key) {
+    return partition_key_join(n_tags, [&](size_t i, std::string* v) {
+        return types[i] != 0 && aux_value_text((char)types[i], values + offs[i], lens[i], v);
+    }, key);
 }
 
 struct PackedChunk {

@@ -44,9 +44,10 @@ int mkh_sample_probs_main(int argc, const char* const* argv) { return sample_mai
 
 // One rank of an interval-sharded `modkit pileup` (SURVEY 8e): every rank is called with the same arguments (plus its own
 // --device); `allreduce` sums a u64 vector over the ranks in place and returns 0 (NCCL through torch.distributed in
-// bench.py / modkit_b200.pileup_main_sharded; any other transport works). It is called exactly twice per run, in the same
+// bench.py / modkit_b200.pileup_main_sharded; any other transport works). Without --partition-tag it is called exactly twice per run, in the same
 // order on every rank: the sampled-probability histograms (u64[4*MKP_HIST_BINS + 2]; thresholds.rs:118-156) and the output slice
-// sizes (u64[world + 2]); with --include-unmapped a third, one-word exchange precedes them.
+// sizes (u64[world + 2]); with --include-unmapped a third, one-word exchange precedes them. With --partition-tag the slice sizes
+// are replaced by the file agreement (agree_file_slices, up to three sums) and one u64[3] sum after the files are made.
 // out_stats (optional, double[20]): total_s, load_s, thresholds_s, gpu_s, write_s, rows (all ranks), positions (all ranks), rows of this
 // rank, base thresholds A C G T (-1 = none), sampler fetch_s, intervals_s, pack_s, kernel_ms, slice_s, pass_s, rowcopy_s.
 static int pileup_main_sharded(int argc, const char* const* argv, bool hemi, int rank, int world, int (*allreduce)(uint64_t*, size_t, void*), void* user, double* out_stats) {
@@ -187,6 +188,31 @@ int mkh_partition_key_of_cells(const uint8_t* cells, uint32_t n_tags, char* out,
     if ((int)k.size() + 1 > cap) return -1;
     memcpy(out, k.c_str(), k.size() + 1);
     return have ? 1 : 0;
+}
+// One rank's side of the file agreement of a sharded --partition-tag run (agree_file_slices): the rank's files are n names
+// (names: n NUL-terminated strings back to back) with sizes[n] bytes; `allreduce` is the rank's u64 sum, as in
+// mkh_pileup_main_sharded. Returns the number of files in the union, or -1. When it is <= cap, out_names gets the sorted union as
+// NUL-terminated strings (names_cap bytes; -2 if they do not fit), and out_offset / out_total each file's offset of this rank and
+// total size.
+int64_t mkh_agree_file_slices(int rank, int world, int (*allreduce)(uint64_t*, size_t, void*), void* user, const char* names, const uint64_t* sizes, uint32_t n,
+                              char* out_names, uint64_t names_cap, uint64_t* out_offset, uint64_t* out_total, uint64_t cap) {
+    try {
+        if (rank < 0 || world < 1 || rank >= world || (world > 1 && !allreduce)) return -1;
+        Collective c;
+        c.rank = rank; c.world = world; c.allreduce_sum = allreduce; c.user = user;
+        std::map<std::string, uint64_t> mine;
+        for (uint32_t i = 0; i < n; i++) { const std::string nm = names; mine[nm] = sizes[i]; names += nm.size() + 1; }
+        const FileSlices fs = agree_file_slices(c, mine);
+        if (fs.names.size() > cap) return (int64_t)fs.names.size();
+        uint64_t at = 0;
+        for (size_t f = 0; f < fs.names.size(); f++) {
+            if (at + fs.names[f].size() + 1 > names_cap) return -2;
+            memcpy(out_names + at, fs.names[f].c_str(), fs.names[f].size() + 1);
+            at += fs.names[f].size() + 1;
+            out_offset[f] = fs.offset[f]; out_total[f] = fs.total[f];
+        }
+        return (int64_t)fs.names.size();
+    } catch (const std::exception& e) { fprintf(stderr, "mkh_agree_file_slices: %s\n", e.what()); return -1; }
 }
 void mkh_bam_close(mkh_bam* b) { delete b; }
 uint32_t mkh_bam_n_refs(const mkh_bam* b) { return (uint32_t)b->reader.ref_names.size(); }

@@ -272,6 +272,50 @@ struct Collective {          // sum over the ranks of a sharded run (in place); 
     }
 };
 
+// The files of a sharded run that writes a directory (--partition-tag). Every rank holds, per file name, the text of its own
+// intervals; a file is the rank-ordered concatenation of those texts. agree_file_slices gives every rank the union of the names
+// (sorted), the total size of each file and this rank's offset in it. Every rank calls it, with whatever map it has (an empty one
+// too). It makes up to three sums, each of the same length on every rank (NCCL requires that): the name-list sizes (world words),
+// the name lists (each rank fills its own window of a zeroed buffer), and the size matrix (files x world). The last two are left
+// out on every rank when no rank has a name.
+struct FileSlices { std::vector<std::string> names; std::vector<uint64_t> offset, total; };
+inline FileSlices agree_file_slices(const Collective& coll, const std::map<std::string, uint64_t>& mine) {
+    const size_t world = (size_t)std::max(1, coll.world), rank = (size_t)coll.rank;
+    // a name list in u64 words: per name its length, then its bytes (zero-padded to whole words)
+    std::vector<uint64_t> list;
+    for (auto& kv : mine) {
+        const std::string& nm = kv.first;
+        list.push_back(nm.size());
+        const size_t at = list.size();
+        list.resize(at + (nm.size() + 7) / 8, 0);
+        memcpy(list.data() + at, nm.data(), nm.size());
+    }
+    std::vector<uint64_t> words(world, 0);
+    words[rank] = list.size();
+    coll.sum(words.data(), words.size());
+    std::vector<uint64_t> all(std::accumulate(words.begin(), words.end(), (uint64_t)0), 0);
+    std::copy(list.begin(), list.end(), all.begin() + (ptrdiff_t)std::accumulate(words.begin(), words.begin() + (ptrdiff_t)rank, (uint64_t)0));
+    if (!all.empty()) coll.sum(all.data(), all.size());           // (every rank knows the size: none sums an empty buffer)
+    std::set<std::string> uni;
+    for (size_t p = 0; p < all.size();) {
+        const size_t len = (size_t)all[p++];
+        if (len > (all.size() - p) * 8) throw std::runtime_error("malformed file-name exchange");
+        uni.insert(std::string((const char*)(all.data() + p), len));
+        p += (len + 7) / 8;
+    }
+    FileSlices fs;
+    fs.names.assign(uni.begin(), uni.end());
+    std::vector<uint64_t> sizes(fs.names.size() * world, 0);           // [file][rank]
+    for (size_t f = 0; f < fs.names.size(); f++) { auto it = mine.find(fs.names[f]); if (it != mine.end()) sizes[f * world + rank] = it->second; }
+    if (!sizes.empty()) coll.sum(sizes.data(), sizes.size());
+    for (size_t f = 0; f < fs.names.size(); f++) {
+        const uint64_t* row = sizes.data() + f * world;
+        fs.offset.push_back(std::accumulate(row, row + rank, (uint64_t)0));
+        fs.total.push_back(std::accumulate(row, row + world, (uint64_t)0));
+    }
+    return fs;
+}
+
 inline void append_packed(const PackedChunk& src, PackedChunk* dst) {
     const uint64_t base = (dst->heap.size() + 15) & ~(uint64_t)15;
     dst->heap.resize(base);
@@ -735,7 +779,7 @@ struct PileupPlan {
         to_dir = !o.partition_tags.empty() || o.bedgraph;
         if (to_dir && o.header) throw std::runtime_error("the argument '--header' cannot be used with '--bedgraph' / '--partition-tag'");
         if (o.bedgraph && o.mixed) throw std::runtime_error("the argument '--mixed-delim' cannot be used with '--bedgraph'");
-        if (sharded && (to_dir || o.host_ingest)) throw std::runtime_error("multi-GPU runs write one bedMethyl file through the device ingest: --bedgraph / --partition-tag / --host-ingest need a single device");
+        if (sharded && (o.bedgraph || o.host_ingest)) throw std::runtime_error("multi-GPU runs write one bedMethyl file through the device ingest, or one per partition: --bedgraph / --host-ingest need a single device");
         if (sharded && (o.out_bed == "-" || o.out_bed == "stdout")) throw std::runtime_error("multi-GPU runs need an output file (ranks write their slices at their offsets)");
         combine_strands = o.combine_strands || o.hemi;        // pileup-hemi: the feeder runs in combine-strands mode
         if (combine_strands && !(o.cpg || !o.motif_parts.empty())) throw std::runtime_error("need to specify either --motif or --cpg to combine strands");
@@ -849,34 +893,52 @@ inline std::vector<ChunkWork> chunk_work(const std::vector<RefInterval>& ivs, si
 }
 
 // With --partition-tag one group of reads per key (each an independent pileup: src/pileup/mod.rs:795-830), in key order, "\1" for
-// the reads without a key; otherwise one group "" of all reads. Device-resident records give their tags on the GPU (mkp_bam_tags).
-inline std::map<std::string, std::vector<RecRef>> partition_groups(mkp_ctx* ctx, const BamReader& reads, const std::vector<std::string>& tags, std::vector<RecRef>&& recs) {
+// the reads without a key; otherwise one group "" of all reads. Device-resident records give their tag values on the GPU
+// (mkp_bam_tag_values, four tags per call, values of any length); `vals` is the host buffer of those values, kept between calls.
+inline std::map<std::string, std::vector<RecRef>> partition_groups(mkp_ctx* ctx, const BamReader& reads, const std::vector<std::string>& tags, std::vector<RecRef>&& recs,
+                                                                   std::vector<uint8_t>* vals) {
     std::map<std::string, std::vector<RecRef>> groups;
     if (tags.empty()) { groups[""] = std::move(recs); return groups; }
     // only alignments the pileup admits create a key (flag filter of the pileup engine, pileup/mod.rs:783-791)
     std::vector<RecRef> adm;
     for (auto& r : recs) if (!((r.flag & (0x4 | 0x100 | 0x200 | 0x400 | 0x800)) || r.l_seq == 0)) adm.push_back(r);
-    std::vector<uint8_t> cells;
     const size_t n_pt = tags.size();
+    // per (record, tag), record-major: aux type, value length, value offset in `vals`
+    std::vector<uint8_t> types;
+    std::vector<uint32_t> lens;
+    std::vector<uint64_t> offs;
     if (reads.on_device && !adm.empty()) {
-        std::vector<uint32_t> ids(adm.size());
-        for (size_t k = 0; k < adm.size(); k++) ids[k] = adm[k].idx;
-        cells.resize(adm.size() * n_pt * MKP_TAG_CELL);
-        // four tags per call (mkp_bam_tags); the cells of a record are laid side by side in tag order
-        std::vector<uint8_t> part;
+        const size_t n = adm.size();
+        std::vector<uint32_t> ids(n);
+        for (size_t k = 0; k < n; k++) ids[k] = adm[k].idx;
+        types.resize(n * n_pt); lens.resize(n * n_pt); offs.resize(n * n_pt);
+        std::vector<uint8_t> pt;
+        std::vector<uint32_t> pl, po;
+        size_t base = 0;                   // the values of earlier calls (tags t0 - 4 ...) come first in `vals`
         for (size_t t0 = 0; t0 < n_pt; t0 += 4) {
             const size_t nt4 = std::min<size_t>(4, n_pt - t0);
             std::string tg;
             for (size_t t = t0; t < t0 + nt4; t++) tg += tags[t];
-            part.resize(adm.size() * nt4 * MKP_TAG_CELL);
-            check_mkp(ctx, mkp_bam_tags(ctx, ids.data(), (uint32_t)ids.size(), tg.c_str(), (uint32_t)nt4, part.data()));
-            for (size_t k = 0; k < adm.size(); k++)
-                memcpy(cells.data() + (k * n_pt + t0) * MKP_TAG_CELL, part.data() + k * nt4 * MKP_TAG_CELL, nt4 * MKP_TAG_CELL);
+            pt.resize(n * nt4); pl.resize(n * nt4); po.resize(n * nt4);
+            uint64_t total = 0;
+            if (vals->size() < base) vals->resize(base);
+            auto call = [&]() {
+                check_mkp(ctx, mkp_bam_tag_values(ctx, ids.data(), (uint32_t)n, tg.c_str(), (uint32_t)nt4, pt.data(), pl.data(), po.data(),
+                                                  vals->data() + base, vals->size() - base, &total));
+            };
+            call();
+            if (vals->size() - base < total) { vals->resize(base + total); call(); }       // sized by the first call
+            for (size_t k = 0; k < n; k++)
+                for (size_t t = 0; t < nt4; t++) {
+                    const size_t q = k * n_pt + t0 + t, j = k * nt4 + t;
+                    types[q] = pt[j]; lens[q] = pl[j]; offs[q] = base + po[j];
+                }
+            base += total;
         }
     }
     for (size_t k = 0; k < adm.size(); k++) {
         std::string key;
-        const bool have = reads.on_device ? partition_key_of_cells(cells.data() + k * n_pt * MKP_TAG_CELL, n_pt, &key)
+        const bool have = reads.on_device ? partition_key_of_values(types.data() + k * n_pt, lens.data() + k * n_pt, offs.data() + k * n_pt, vals->data(), n_pt, &key)
                                           : partition_key_of(reads.rec(adm[k]), adm[k].size, tags, &key);
         groups[have ? key : std::string("\1")].push_back(adm[k]);
     }
@@ -935,6 +997,7 @@ inline void device_stage(mkp_ctx* ctx, const BamReader& reads, const PileupOptio
     const std::vector<RefInterval>& ivs = plan.ivs;
     PackedChunk pc;
     std::vector<uint32_t> fpos, fneg;
+    std::vector<uint8_t> tag_vals;
     for (size_t c0 = 0, c1; c0 < ivs.size(); c0 = c1) {
         c1 = chunk_end(ivs, c0, o.chunk_bp);
         if (ivs[c1 - 1].end <= ivs[c0].start) continue;
@@ -953,7 +1016,7 @@ inline void device_stage(mkp_ctx* ctx, const BamReader& reads, const PileupOptio
             std::vector<uint32_t> starts;
             if (o.hemi) for (size_t k = i0; k < i1; k++) starts.push_back(ivs[k].start);
             bool focus_done = false;
-            for (auto& grp : partition_groups(ctx, reads, o.partition_tags, std::move(wk.recs))) {
+            for (auto& grp : partition_groups(ctx, reads, o.partition_tags, std::move(wk.recs), &tag_vals)) {
                 const auto ta = clk::now();
                 pc.clear();
                 if (reads.on_device) pc.recs = grp.second;
@@ -984,6 +1047,8 @@ class PileupWriter {
     std::vector<std::string> parts_;                          // per formatting worker (capacity kept from chunk to chunk)
     std::vector<std::map<std::string, std::string>> routed_;  // per formatting worker, to a directory: file name -> text
     std::vector<std::string> slice_;   // sharded: the header (rank 0), then the formatted parts in order
+    const bool to_dir_;
+    std::map<std::string, std::vector<std::string>> dir_slices_;   // sharded, to a directory: file name -> its formatted parts in order
     static bool pwrite_all(int fd, const std::string& text, uint64_t offset) {
         for (size_t done = 0; done < text.size();) {
             const ssize_t w = pwrite(fd, text.data() + done, text.size() - done, (off_t)(offset + done));
@@ -998,8 +1063,14 @@ class PileupWriter {
         return f;
     }
 public:
-    PileupWriter(const PileupOptions& o, bool to_dir, const Collective& coll) : path_(o.out_bed), coll_(coll) {
-        if (coll.world > 1) {
+    PileupWriter(const PileupOptions& o, bool to_dir, const Collective& coll) : path_(o.out_bed), coll_(coll), to_dir_(to_dir) {
+        if (coll.world > 1 && to_dir) {
+            if (coll.rank == 0) {             // the files are made at the end, once the ranks agree on them
+                std::error_code ec;
+                std::filesystem::create_directories(path_, ec);
+                if (ec) throw std::runtime_error("failed to create output directory " + path_);
+            }
+        } else if (coll.world > 1) {
             if (coll.rank == 0) {
                 FILE* f = fopen(path_.c_str(), "w");     // created (and truncated) by rank 0 before the first exchange
                 if (!f) throw std::runtime_error("failed to make output file");
@@ -1047,7 +1118,11 @@ public:
             if (coll_.world > 1) { if (!parts_[t].empty()) slice_.push_back(std::move(parts_[t])); }
             else if (fd_ >= 0) pos_ += parts_[t].size();
             else if (out_) fwrite(parts_[t].data(), 1, parts_[t].size(), out_);
-            for (auto& kv : routed_[t]) if (!kv.second.empty()) fwrite(kv.second.data(), 1, kv.second.size(), file(kv.first));
+            for (auto& kv : routed_[t]) {
+                if (kv.second.empty()) continue;
+                if (coll_.world > 1) dir_slices_[kv.first].push_back(std::move(kv.second));
+                else fwrite(kv.second.data(), 1, kv.second.size(), file(kv.first));
+            }
         }
     }
 
@@ -1057,6 +1132,7 @@ public:
         if (out_) { if (out_ != stdout) fclose(out_); else fflush(out_); out_ = nullptr; }
         if (coll_.world <= 1) { S->rows_total = S->rows; S->positions_total = S->positions; return; }
         const auto tw = std::chrono::steady_clock::now();
+        if (to_dir_) { finish_dir(pool, S); S->write_s += secs_between(tw, std::chrono::steady_clock::now()); return; }
         std::vector<uint64_t> sizes((size_t)coll_.world + 2, 0), at(slice_.size());
         for (auto& s : slice_) sizes[coll_.rank] += s.size();
         sizes[coll_.world] = S->rows; sizes[(size_t)coll_.world + 1] = S->positions;
@@ -1072,7 +1148,44 @@ public:
         S->rows_total = sizes[coll_.world]; S->positions_total = sizes[(size_t)coll_.world + 1];
         S->write_s += secs_between(tw, std::chrono::steady_clock::now());
     }
-    void release_buffers() { parts_.clear(); parts_.shrink_to_fit(); slice_.clear(); slice_.shrink_to_fit(); }
+    // Sharded, to a directory: the ranks agree on the files and on every rank's offset in each (agree_file_slices); rank 0 makes
+    // (or truncates) every file that gets text, the next exchange holds the others back until that is done, then every rank writes
+    // its parts in place. Files no rank has text for are not touched, as with one device.
+    void finish_dir(WorkerPool& pool, RunSummary* S) {
+        std::map<std::string, uint64_t> mine;
+        for (auto& kv : dir_slices_) { uint64_t n = 0; for (auto& part : kv.second) n += part.size(); mine[kv.first] = n; }
+        const FileSlices fs = agree_file_slices(coll_, mine);
+        uint64_t made_fail = 0;
+        if (coll_.rank == 0)
+            for (size_t f = 0; f < fs.names.size(); f++) {
+                if (!fs.total[f]) continue;
+                const int fd = ::open((path_ + "/" + fs.names[f]).c_str(), O_WRONLY | O_CREAT | O_TRUNC, 0666);
+                if (fd < 0) { made_fail = 1; break; }
+                ::close(fd);
+            }
+        uint64_t done[3] = {made_fail, S->rows, S->positions};
+        coll_.sum(done, 3);
+        if (done[0]) throw std::runtime_error("failed to make output files in " + path_);
+        struct Job { int fd; const std::string* text; uint64_t at; };
+        std::vector<Job> jobs;
+        std::vector<int> fds;
+        bool open_failed = false;
+        for (size_t f = 0; f < fs.names.size() && !open_failed; f++) {
+            auto it = dir_slices_.find(fs.names[f]);
+            if (it == dir_slices_.end()) continue;
+            const int fd = ::open((path_ + "/" + fs.names[f]).c_str(), O_WRONLY);
+            if (fd < 0) { open_failed = true; break; }
+            fds.push_back(fd);
+            uint64_t at = fs.offset[f];
+            for (auto& part : it->second) { jobs.push_back({fd, &part, at}); at += part.size(); }
+        }
+        std::atomic<bool> failed{open_failed};
+        if (!open_failed) pool.run((int)jobs.size(), [&](int k) { if (!failed && !pwrite_all(jobs[k].fd, *jobs[k].text, jobs[k].at)) failed = true; });
+        for (int fd : fds) ::close(fd);
+        if (failed) throw std::runtime_error("failed to write output files in " + path_);
+        S->rows_total = done[1]; S->positions_total = done[2];
+    }
+    void release_buffers() { parts_.clear(); parts_.shrink_to_fit(); slice_.clear(); slice_.shrink_to_fit(); dir_slices_.clear(); }
 };
 
 // The rows of one chunk as text (position sorted: every interval gets its slice; intervals are formatted in parallel); row count

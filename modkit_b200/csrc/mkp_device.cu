@@ -70,6 +70,8 @@ struct mkp_ctx {
     DevBuf d_obs_word, d_slots, d_row_counts, d_row_prefix, d_rows, d_hist, d_take;
     // device ingest (BGZF file, inflated BAM stream, record table, slicing scratch)
     DevBuf d_file, d_members, d_bam, d_seeds, d_seg_counts, d_seg_base, d_recs, d_ids, d_plan, d_need, d_totals, d_slab_work;
+    // mkp_bam_tag_values: per (record, tag) type, length, offset in the values and in the inflated stream; the packed values
+    DevBuf d_tag_type, d_tag_len, d_tag_off, d_tag_src, d_tag_val;
     uint64_t bam_len = 0;
     size_t n_records = 0;
     bool inflate_attr_set = false;
@@ -121,9 +123,12 @@ struct PassScratch {
     uint32_t tile_counter;                   // TileDev::tile_counter
     uint32_t tag_overflow;                   // k_tag_values
     uint32_t n_items;                        // upload: work items of k_count_bases (scan total)
+    uint32_t tag_bytes;                      // mkp_bam_tag_values: scan total of the value lengths
+    unsigned long long tag_bytes_wide;       // the same sum in 64 bits (a total past 4 GiB is refused, not wrapped)
 };
-static_assert(sizeof(PassScratch) == 336 && offsetof(PassScratch, n_states) == 272 && offsetof(PassScratch, work) == 288 &&
-              offsetof(PassScratch, read_counter) == 320 && offsetof(PassScratch, tag_overflow) == 328 && offsetof(PassScratch, n_items) == 332,
+static_assert(sizeof(PassScratch) == 352 && offsetof(PassScratch, n_states) == 272 && offsetof(PassScratch, work) == 288 &&
+              offsetof(PassScratch, read_counter) == 320 && offsetof(PassScratch, tag_overflow) == 328 && offsetof(PassScratch, n_items) == 332 &&
+              offsetof(PassScratch, tag_bytes) == 336 && offsetof(PassScratch, tag_bytes_wide) == 344,
               "d_small layout");
 
 static int fail(mkp_ctx* c, const std::string& m, int code = -1) { if (c) c->err = m; return code; }
@@ -1176,6 +1181,49 @@ int mkp_bam_tags(mkp_ctx* ctx, const uint32_t* rec_ids, uint32_t n, const char* 
     PassScratch h;
     if (int rc = read_scratch(ctx, &h)) return rc;
     if (h.tag_overflow) return fail(ctx, "a partition tag value is longer than 253 bytes: use --host-ingest for this file");
+    return 0;
+}
+
+int mkp_bam_tag_values(mkp_ctx* ctx, const uint32_t* rec_ids, uint32_t n, const char* tags, uint32_t n_tags,
+                       uint8_t* types, uint32_t* lens, uint32_t* offs, uint8_t* values, uint64_t cap, uint64_t* total) {
+    if (!ctx || !tags || !total || n_tags == 0 || n_tags > 4 || (n && (!rec_ids || !types || !lens || !offs))) return -1;
+    if (!ctx->bam_len) return fail(ctx, "mkp_bam_load was not called");
+    CK(cudaSetDevice(ctx->device));
+    *total = 0;
+    if (!n) return 0;
+    const size_t m = (size_t)n * n_tags;
+    if (m > UINT32_MAX) return fail(ctx, "too many (record, tag) pairs in one call");
+    cudaStream_t st = ctx->stream;
+    for (uint32_t i = 0; i < n; i++) if (rec_ids[i] >= ctx->n_records) return fail(ctx, "record id out of range");
+    CK(ctx->d_ids.ensure((size_t)n * 4));
+    CK(ctx->d_tag_type.ensure(m));
+    CK(ctx->d_tag_len.ensure(m * 4));
+    CK(ctx->d_tag_off.ensure(m * 4));
+    CK(ctx->d_tag_src.ensure(m * 8));
+    CK(ctx->d_small.ensure(sizeof(PassScratch)));
+    PassScratch* const s = ctx->d_small.as<PassScratch>();
+    uint32_t pk[4] = {0, 0, 0, 0};
+    for (uint32_t t = 0; t < n_tags; t++) pk[t] = (uint32_t)(uint8_t)tags[2 * t] | ((uint32_t)(uint8_t)tags[2 * t + 1] << 8);
+    CK(cudaMemcpyAsync(ctx->d_ids.p, rec_ids, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(&s->tag_bytes_wide, 0, sizeof s->tag_bytes_wide, st));
+    launch(ctx, k_tag_value_lens, (n + 7) / 8, 256, 0, st, ctx->d_bam.as<uint8_t>(), ctx->d_recs.as<mkp_bam_rec>(), ctx->d_ids.as<uint32_t>(), n,
+           pk[0] | (pk[1] << 16), pk[2] | (pk[3] << 16), n_tags, ctx->d_tag_type.as<uint8_t>(), ctx->d_tag_len.as<uint32_t>(), ctx->d_tag_src.as<uint64_t>(),
+           &s->tag_bytes_wide);
+    if (int rc = exclusive_scan_u32(ctx, ctx->d_tag_len.as<uint32_t>(), (uint32_t)m, ctx->d_tag_off.as<uint32_t>(), &s->tag_bytes)) return rc;
+    CK(cudaMemcpyAsync(types, ctx->d_tag_type.p, m, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(lens, ctx->d_tag_len.p, m * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(offs, ctx->d_tag_off.p, m * 4, cudaMemcpyDeviceToHost, st));
+    PassScratch h;
+    if (int rc = read_scratch(ctx, &h)) return rc;
+    if (h.tag_bytes_wide > UINT32_MAX) return fail(ctx, "the partition tag values of one call exceed 4 GiB");
+    *total = h.tag_bytes_wide;
+    if (!values || cap < *total || !*total) return 0;
+    CK(ctx->d_tag_val.ensure(*total));
+    launch(ctx, k_tag_value_copy, (uint32_t)((m + 7) / 8), 256, 0, st, ctx->d_bam.as<uint8_t>(), ctx->d_tag_len.as<uint32_t>(), ctx->d_tag_off.as<uint32_t>(),
+           ctx->d_tag_src.as<uint64_t>(), (uint32_t)m, ctx->d_tag_val.as<uint8_t>());
+    CK(cudaMemcpyAsync(values, ctx->d_tag_val.p, *total, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    CK(cudaGetLastError());
     return 0;
 }
 

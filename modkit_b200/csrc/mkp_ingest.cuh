@@ -664,4 +664,55 @@ __global__ void __launch_bounds__(256) k_tag_values(const uint8_t* __restrict__ 
     }
 }
 
+// ---- the same values without a length limit (mkp_bam_tag_values): a warp per selected record finds up to 4 tags and writes,
+//      per item k = i * n_tags + t, the aux type (0: absent or a B array), the value length and the value's offset in the
+//      inflated stream; the lengths are then scanned and k_tag_value_copy packs the values at their offsets.
+__global__ void __launch_bounds__(256) k_tag_value_lens(const uint8_t* __restrict__ bam, const mkp_bam_rec* __restrict__ recs, const uint32_t* __restrict__ ids, uint32_t n,
+                                                        uint32_t tags_packed_lo, uint32_t tags_packed_hi, uint32_t n_tags,
+                                                        uint8_t* __restrict__ types, uint32_t* __restrict__ lens, uint64_t* __restrict__ src, unsigned long long* total) {
+    const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (i >= n) return;
+    const mkp_bam_rec rc = recs[ids[i]];
+    const uint8_t* r = bam + rc.off;
+    const uint32_t l_name = r[8], n_cigar = ld_u16(r + 12);
+    const int32_t ls = (int32_t)ld_u32(r + 16);
+    const uint64_t l_seq = ls > 0 ? (uint64_t)ls : 0;
+    const uint64_t aux = rc.off + 32 + l_name + 4ull * n_cigar + (l_seq + 1) / 2 + l_seq, rend = rc.off + rc.size;
+    const uint16_t want[4] = {(uint16_t)(tags_packed_lo & 0xffffu), (uint16_t)(n_tags > 1 ? tags_packed_lo >> 16 : 0xffffu),
+                              (uint16_t)(n_tags > 2 ? tags_packed_hi & 0xffffu : 0xffffu), (uint16_t)(n_tags > 3 ? tags_packed_hi >> 16 : 0xffffu)};
+    AuxHitDev hit[4];
+    aux_scan_warp<4>(bam, aux < rend ? aux : rend, rend, want, hit, lane);
+    if (lane) return;
+    uint64_t sum = 0;
+#pragma unroll
+    for (uint32_t t = 0; t < 4; t++) {
+        if (t >= n_tags) break;
+        const AuxHitDev h = hit[t];
+        uint32_t len = 0;
+        uint8_t ty = h.found ? (uint8_t)h.type : 0;
+        switch (ty) {
+            case 'Z': case 'H': len = h.n; break;
+            case 'A': case 'c': case 'C': len = 1; break;
+            case 's': case 'S': len = 2; break;
+            case 'i': case 'I': case 'f': len = 4; break;
+            default: ty = 0;                                     // B arrays are not stringable: the tag counts as missing
+        }
+        const size_t k = (size_t)i * n_tags + t;
+        types[k] = ty; lens[k] = len; src[k] = h.p;
+        sum += len;
+    }
+    if (sum) atomicAdd(total, (unsigned long long)sum);
+}
+
+// warp per item: the value bytes to out[offs[k] ..)
+__global__ void __launch_bounds__(256) k_tag_value_copy(const uint8_t* __restrict__ bam, const uint32_t* __restrict__ lens, const uint32_t* __restrict__ offs,
+                                                        const uint64_t* __restrict__ src, uint32_t m, uint8_t* __restrict__ out) {
+    const uint32_t k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (k >= m) return;
+    const uint32_t len = lens[k];
+    const uint8_t* s = bam + src[k];
+    uint8_t* o = out + offs[k];
+    for (uint32_t b = lane; b < len; b += 32) o[b] = s[b];
+}
+
 }  // namespace mkp

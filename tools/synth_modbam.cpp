@@ -5,6 +5,8 @@
 //
 //   synth_modbam --out PREFIX [--contig NAME:LEN]... [--coverage 30] [--seed 20260924] [--mods m|hm|hma]
 //                [--mean-len 12000] [--level 1] [--threads 8] [--combined-hm] [--implicit] [--odd-records] [--partition-tags [--long-rg]]
+//                [--contig-tag TAG]  (every read carries TAG:Z:<its contig's name>: a partition value held by the reads of one contig)
+//                [--long-tags]  (RG:Z and XH:H values of 254, 255, 256, 1000 or 70000 bytes, by read id; every 7th read has neither)
 //                [--start-grid G]  (read starts snapped to multiples of G: stacks of reads sharing a start, for --max-depth)
 //                [--region-only START-END]   (only reads overlapping the window; reference still full length)
 //                [--duplex]  (duplex basecalls: G-h?/G-m? lists for the opposite strand's C of every CpG beside the C+ lists, T-a?
@@ -52,6 +54,8 @@ struct Opts {
     bool combined_hm = false, implicit = false, odd = false, duplex = false;
     bool ptags = false;    // --partition-tags: RG:Z (A/B/C or absent), HP (C or i, or absent), XF:f on some reads
     bool long_rg = false;  // --long-rg: the RG values are long run ids (ONT style, ~80 characters) ending in A/B/C
+    std::string contig_tag;    // --contig-tag TAG: TAG:Z:<contig name> on every read
+    bool long_tags = false;    // --long-tags: RG:Z and XH:H values longer than 253 bytes (none draws from the random streams)
     int64_t win_start = -1, win_end = -1;
     uint32_t start_grid = 0;   // --start-grid G: read starts snapped down to multiples of G (amplicon-like stacks of reads with one start)
 };
@@ -283,6 +287,20 @@ static void make_read(const Opts& o, const Contig& c, int32_t tid, uint32_t star
         else if (u2 < 0.8) { v.push_back('H'); v.push_back('P'); v.push_back('i'); put<int32_t>(v, 3); }
         if (u3 < 0.3) { v.push_back('X'); v.push_back('F'); v.push_back('f'); const float f = u3 < 0.1 ? 0.1f : (u3 < 0.2 ? 2.5f : 1.0f / 3.0f); uint32_t b; memcpy(&b, &f, 4); put<uint32_t>(v, b); }
     }
+    if (!o.contig_tag.empty()) {
+        v.push_back((uint8_t)o.contig_tag[0]); v.push_back((uint8_t)o.contig_tag[1]); v.push_back('Z');
+        v.insert(v.end(), o.contigs[tid].first.begin(), o.contigs[tid].first.end()); v.push_back(0);
+    }
+    if (o.long_tags && read_id % 7 != 6) {
+        static const uint32_t LENS[5] = {254, 255, 256, 1000, 70000};
+        const uint32_t lr = LENS[read_id % 5], lh = LENS[(read_id / 5) % 5];
+        v.push_back('R'); v.push_back('G'); v.push_back('Z');
+        for (uint32_t k = 0; k + 1 < lr; k++) v.push_back((uint8_t)('a' + k % 26));
+        v.push_back((uint8_t)("AB"[(read_id / 25) % 2])); v.push_back(0);
+        v.push_back('X'); v.push_back('H'); v.push_back('H');
+        for (uint32_t k = 0; k < lh; k++) v.push_back((uint8_t)"0123456789ABCDEF"[(k + read_id % 3) % 16]);
+        v.push_back(0);
+    }
     const uint32_t bs = (uint32_t)(v.size() - rec0 - 4);
     memcpy(v.data() + rec0, &bs, 4);
     out->recs.push_back({tid, (int32_t)start, (int32_t)ref_end, flag, bs + 4});
@@ -309,11 +327,14 @@ int main(int argc, char** argv) {
         else if (a == "--duplex") o.duplex = true;
         else if (a == "--partition-tags") o.ptags = true;
         else if (a == "--long-rg") o.long_rg = true;
+        else if (a == "--contig-tag") { o.contig_tag = val(); if (o.contig_tag.size() != 2) { fprintf(stderr, "--contig-tag needs a two-letter tag\n"); exit(2); } }
+        else if (a == "--long-tags") o.long_tags = true;
         else if (a == "--start-grid") o.start_grid = (uint32_t)std::stoul(val());
         else if (a == "--region-only") { std::string s = val(); auto d = s.find('-'); o.win_start = std::stoll(s.substr(0, d)); o.win_end = std::stoll(s.substr(d + 1)); }
         else { fprintf(stderr, "unknown flag %s\n", a.c_str()); return 2; }
     }
     if (o.contigs.empty()) o.contigs.push_back({"syn1", 1000000});
+    if (o.long_tags && o.ptags) { fprintf(stderr, "--long-tags and --partition-tags both write RG\n"); return 2; }
     const int nt = std::max(1, o.threads);
 
     // ---- reference: uniform ACGT, CpG observed/expected 0.25, per-site methylation ~ Beta(0.5,0.5)
