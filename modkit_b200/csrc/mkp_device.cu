@@ -1275,6 +1275,17 @@ int mkp_debug_parse_clocks(unsigned long long* out, int n, int reset) {
 }
 #endif
 
+#ifdef MKP_RESOLVE_CLOCKS
+// Measurement builds only: the fast k_resolve phase counters (mkp_kernels.cuh, g_resolve_clk), as mkp_debug_parse_clocks.
+int mkp_debug_resolve_clocks(unsigned long long* out, int n, int reset) {
+    unsigned long long v[RCLK_N];
+    if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(v, g_resolve_clk, sizeof v) != cudaSuccess) return -1;
+    for (int k = 0; k < n && k < RCLK_N; k++) out[k] = v[k];
+    if (reset) { memset(v, 0, sizeof v); if (cudaMemcpyToSymbol(g_resolve_clk, v, sizeof v) != cudaSuccess) return -1; }
+    return RCLK_N;
+}
+#endif
+
 #ifdef MKP_COUNT_CLOCKS
 // Measurement builds only: the k_count_bases item log (mkp_kernels.cuh, g_count_clk) of the current device. out == nullptr:
 // (re)arm a zeroed log of n records; else copy the first n records (32 bytes each) of the log to out. Returns 0.

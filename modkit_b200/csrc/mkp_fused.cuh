@@ -521,7 +521,7 @@ __device__ __forceinline__ void fused_read(const FusedDev& F, FzWarp& W, StateCa
                 const uint8_t* m1 = ml + T.ml_off[ga[b]];
                 bool bad = false;
                 for (uint32_t j = lane; j < n; j += 32) {
-                    const float p0 = __fdiv_rn(__fadd_rn((float)m0[j], 0.5f), 256.0f), p1 = __fdiv_rn(__fadd_rn((float)m1[j], 0.5f), 256.0f);
+                    const float p0 = ml_prob(m0[j]), p1 = ml_prob(m1[j]);
                     if (__fadd_rn(p0, p1) > 1.01f) bad = true;
                 }
                 if (__any_sync(FULL, bad)) err = true;
@@ -663,19 +663,13 @@ __device__ __forceinline__ void fused_read(const FusedDev& F, FzWarp& W, StateCa
                                 const uint4 wr = F.rec[rel >> 5];
                                 if (((wr.x | wr.y) >> (rel & 31)) & 1u) {
                                     // probabilities -> collapse -> call (src/mod_bam.rs:558-600, src/threshold_mod_caller.rs:28-63)
-                                    float p0 = __fdiv_rn(__fadd_rn((float)m0[(size_t)j * two], 0.5f), 256.0f), p1 = 0.f;
+                                    float p0 = ml_prob(m0[(size_t)j * two]), p1 = 0.f;
                                     uint32_t c0 = T.code[lp][0], c1 = 0;
                                     int n2c = 1;
-                                    if (two == 2) { p1 = __fdiv_rn(__fadd_rn((float)m0[(size_t)j * 2 + 1], 0.5f), 256.0f); c1 = T.code[lp][1]; n2c = 2; }
-                                    else if (ga[b] >= 0) { p1 = __fdiv_rn(__fadd_rn((float)m1[j], 0.5f), 256.0f); c1 = T.code[ga[b]][0]; n2c = 2; }
+                                    if (two == 2) { p1 = ml_prob(m0[(size_t)j * 2 + 1]); c1 = T.code[lp][1]; n2c = 2; }
+                                    else if (ga[b] >= 0) { p1 = ml_prob(m1[j]); c1 = T.code[ga[b]][0]; n2c = 2; }
                                     uint32_t s0 = gs0[b], s1 = gs1[b];
-                                    if (c_par.numeric_mode == 2) {
-                                        const uint32_t drop = c_par.collapse_code;
-                                        if (n2c == 1) { if (c0 == drop) n2c = 0; else p0 = __fadd_rn(p0, __fdiv_rn(0.f, 2.0f)); }
-                                        else if (c0 == drop) { c0 = c1; p0 = __fadd_rn(p1, __fdiv_rn(p0, 2.0f)); n2c = 1; }
-                                        else if (c1 == drop) { p0 = __fadd_rn(p0, __fdiv_rn(p1, 2.0f)); n2c = 1; }
-                                        else { const float sh = __fdiv_rn(0.f, 3.0f); p0 = __fadd_rn(p0, sh); p1 = __fadd_rn(p1, sh); }
-                                    }
+                                    if (c_par.numeric_mode == 2) redistribute2(c_par.collapse_code, c0, p0, c1, p1, n2c);
                                     if (n2c == 2) {        // FxHashMap iteration order of the two codes
                                         const uint32_t h0 = bucket4(c0), h1 = bucket4(c1);
                                         if (h0 != h1 ? (h1 < h0) : (h0 == 3)) { const uint32_t tc = c0; c0 = c1; c1 = tc; const float tp = p0; p0 = p1; p1 = tp; const uint32_t ts = s0; s0 = s1; s1 = ts; }

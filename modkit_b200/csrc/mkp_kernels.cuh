@@ -260,6 +260,18 @@ struct Items {
 };
 // low two bits of the Fx hash: K = 1 (mod 4), rotl(K,5) = 2 (mod 4)
 __device__ __forceinline__ uint32_t bucket4(uint32_t c) { return (c & 0x80000000u) ? ((2u ^ c) & 3u) : (c & 3u); }
+// ML byte -> probability, (b + 0.5) / 256 (mod_bam.rs). b + 0.5 is exact in float and 256 is a power of two, so the product
+// by 2^-8 is the same real number as the quotient and rounds to the same bits, without a division.
+__device__ __forceinline__ float ml_prob(uint32_t b) { return __fmul_rn(__fadd_rn((float)b, 0.5f), 0x1p-8f); }
+// CollapseMethod::ReDistribute (src/mod_bam.rs:558-600) of at most two codes: the dropped code's probability is shared as
+// marginal / (n_other + 1). With two codes that is p / 2, which p * 0.5 gives exactly (the same real number); when no code is
+// dropped the share is 0 / k = +0, and p + 0 is p for every p >= 0, so that add is left out.
+__device__ __forceinline__ float half_share(float p) { return __fmul_rn(p, 0.5f); }
+__device__ __forceinline__ void redistribute2(uint32_t drop, uint32_t& c0, float& p0, uint32_t c1, float p1, int& n2c) {
+    if (n2c == 1) { if (c0 == drop) n2c = 0; }
+    else if (c0 == drop) { c0 = c1; p0 = __fadd_rn(p1, half_share(p0)); n2c = 1; }
+    else if (c1 == drop) { p0 = __fadd_rn(p0, half_share(p1)); n2c = 1; }
+}
 __device__ __noinline__ void iter_order_slow(const Items& it, int* ord) {
     ProbMap m;
     m.init();
@@ -292,22 +304,27 @@ __device__ __forceinline__ void redistribute_items(const Items& in, const int* o
     out.n = 0;
     for (int k = 0; k < in.n; k++) { const int i = ord[k]; if (in.code[i] != drop) out.push(in.code[i], __fadd_rn(in.p[i], share)); }
 }
+// threshold of mod code c at canonical base tb: the code's own, else the base's any-mod ("C") one, else base_thr
+__device__ __forceinline__ float mod_threshold(uint32_t c, int tb, float base_thr) {
+    float thr = base_thr;
+    if (c_par.n_mod_thr) {
+        const uint32_t any_code = (uint32_t)("ACGT"[tb]);
+        bool found = false;
+        for (uint32_t t = 0; t < c_par.n_mod_thr && !found; t++) if (c_par.mod_code[t] == c) { thr = c_par.mod_thr[t]; found = true; }
+        for (uint32_t t = 0; t < c_par.n_mod_thr && !found; t++) if (c_par.mod_code[t] == any_code) { thr = c_par.mod_thr[t]; found = true; }
+    }
+    return thr;
+}
 // MultipleThresholdModCaller::call (src/threshold_mod_caller.rs:28-63): 0 filtered, 1 canonical, 2 modified (*code)
 __device__ __forceinline__ int make_call_items(const Items& it, const int* ord, int tb, uint32_t* code) {
     bool have = false;
     float best = 0.f;
     int kind = 0;
-    const uint32_t any_code = (uint32_t)("ACGT"[tb]);
     const float base_thr = c_par.base_set[tb] ? c_par.base_thr[tb] : c_par.default_thr;
     for (int k = 0; k < it.n; k++) {
         const int i = ord[k];
         const uint32_t c = it.code[i];
-        float thr = base_thr;
-        if (c_par.n_mod_thr) {
-            bool found = false;
-            for (uint32_t t = 0; t < c_par.n_mod_thr && !found; t++) if (c_par.mod_code[t] == c) { thr = c_par.mod_thr[t]; found = true; }
-            for (uint32_t t = 0; t < c_par.n_mod_thr && !found; t++) if (c_par.mod_code[t] == any_code) { thr = c_par.mod_thr[t]; found = true; }
-        }
+        const float thr = mod_threshold(c, tb, base_thr);
         const float pm = it.p[i];
         if (pm >= thr && (!have || pm >= best)) { have = true; best = pm; kind = 2; *code = c; }
     }
@@ -391,8 +408,11 @@ __device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t* P, uint32_t 
 #ifndef MKP_MINB_PARSE
 #define MKP_MINB_PARSE 9
 #endif
+// fast k_resolve: 7 blocks of 128 threads = 72 registers, 140 / 80 bytes of spills. Before its loads were issued together, on an
+// H100 it took 1.44 ms per pass on the profile chunk at 7 blocks, against 1.76 at 8 (64 registers) and 1.98 at 9
+// (profiles/resolve_ptxas.txt, profiles/README.md)
 #ifndef MKP_MINB_RESOLVE_FAST
-#define MKP_MINB_RESOLVE_FAST 8
+#define MKP_MINB_RESOLVE_FAST 7
 #endif
 #ifndef MKP_MINB_RESOLVE
 #define MKP_MINB_RESOLVE 7
@@ -421,6 +441,33 @@ __device__ unsigned long long g_parse_clk[PCLK_N];
 #define PCLK(k) do {} while (0)
 #define PCLK_COUNT(k, n) do {} while (0)
 #define PCLK_FLUSH do {} while (0)
+#endif
+// MKP_RESOLVE_CLOCKS=1 (measurement builds only): every warp of the fast k_resolve<MODE_PILEUP> sums clock64() deltas per phase
+// over the reads it handles and adds them into g_resolve_clk at exit: [0] queue + header + list table, [1] CIGAR prefix,
+// [2] query -> op table, [3] per-entry resolve (ML -> call), [4] projection + emit, [5] commit, [6] reads, [7] list entries.
+// Each round of 32 entries splits at the slowest lane's end of the call: lanes run the call and the projection in turn, and the
+// warp moves on when its last lane is done. Read back by mkp_debug_resolve_clocks.
+#ifdef MKP_RESOLVE_CLOCKS
+constexpr int RCLK_N = 8;
+__device__ unsigned long long g_resolve_clk[RCLK_N];
+#define RCLK_ON (FAST_ONLY && MODE == MODE_PILEUP)
+#define RCLK_INIT __shared__ unsigned long long s_rclk[4][RCLK_N]; unsigned long long* rclk = s_rclk[wib]; \
+    if (lane < RCLK_N) rclk[lane] = 0; __syncwarp(); unsigned long long rclk_t = clock64(), rclk_mid = 0
+#define RCLK(k) do { if (RCLK_ON) { const unsigned long long t_ = clock64(); if (lane == 0) rclk[k] += t_ - rclk_t; rclk_t = t_; } } while (0)
+#define RCLK_COUNT(k, n) do { if (RCLK_ON && lane == 0) rclk[k] += (n); } while (0)
+#define RCLK_MARK do { if (RCLK_ON) rclk_mid = clock64(); } while (0)
+#define RCLK_ROUND do { if (RCLK_ON) { \
+    const unsigned long long t_ = clock64(); \
+    const uint32_t d_ = __reduce_max_sync(FULL, rclk_mid > rclk_t ? (uint32_t)min(rclk_mid - rclk_t, t_ - rclk_t) : 0u); \
+    if (lane == 0) { rclk[3] += d_; rclk[4] += t_ - rclk_t - d_; } rclk_t = t_; rclk_mid = 0; } } while (0)
+#define RCLK_FLUSH do { if (RCLK_ON) { __syncwarp(); if (lane < RCLK_N) atomicAdd(&g_resolve_clk[lane], rclk[lane]); } } while (0)
+#else
+#define RCLK_INIT do {} while (0)
+#define RCLK(k) do {} while (0)
+#define RCLK_COUNT(k, n) do {} while (0)
+#define RCLK_MARK do {} while (0)
+#define RCLK_ROUND do {} while (0)
+#define RCLK_FLUSH do {} while (0)
 #endif
 // SEQ per lane and round of k_parse's streaming select, in uint4 (32 bases each). On an H100, 2 took 1.95 ms per pass on the
 // profile chunk and 4 took 2.07 (profiles/README.md): wider blocks cost more in the token lookup than they save in rounds.
@@ -970,6 +1017,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
     ListTab& T = s_tab[wib];
     StateCache scache;
     scache.init();
+    RCLK_INIT;
     uint32_t* const gcq = C.scr_cq + (size_t)gw * (C.max_ncigar + 4);
     uint32_t* const gcr = C.scr_cr + (size_t)gw * (C.max_ncigar + 4);
 
@@ -1034,6 +1082,8 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
             if (lane == 0) C.slow_list[atomicAdd(C.work + 4, 1u)] = ri;
             continue;
         }
+        RCLK(0);
+        RCLK_COUNT(6, 1);
         // CIGAR prefix: query / reference start of every op; four ops per lane (one 16-byte load), 128 per round
         const uint32_t nc = h.n_cigar;
         uint32_t q_total = 0;
@@ -1070,6 +1120,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
             q_total = qc;
         }
         __syncwarp();
+        RCLK(1);
         // query -> op table: qt[t] = the op that holds query base t << shift (the largest i with cq[i] <= that base)
         uint32_t qt_shift = 7;
         while (qt_shift < 31 && (q_total >> qt_shift) >= (uint32_t)QT_CAP) qt_shift++;
@@ -1083,6 +1134,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
             if (lane == 0) qt[(q_total + B - 1) >> qt_shift] = (uint16_t)(nc - 1);
         }
         __syncwarp();
+        RCLK(2);
         uint32_t* P = C.P + meta.entry_off;
         // ---- phase 4: resolve entries -> calls ---------------------------------------------------
         uint32_t n_calls = 0, n_hist = 0;
@@ -1106,6 +1158,37 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                 for (uint32_t l2 = nl; l2-- > l + 1;) if (T.strand[l2] == st && T.n_delta[l2]) lnext = l2;
                 uint32_t cnt_next = 0;
                 const uint32_t calls_before = n_calls;
+                RCLK_COUNT(7, n);
+                // Register-only path: an entry holds the list's first code c0, and either nothing else ("single") or the
+                // pair code pc1 ("pair": the list's second code, or the code of lnext where lnext holds the entry). A pair
+                // code equal to c0 adds into c0's probability, so the entry stays single. Whatever depends only on the
+                // list is worked out here, once, for both shapes: the codes left after ReDistribute in FxHash order
+                // (k-th out code = (sel ^ k) ? pc1 : c0), their thresholds, and (on first use, per lane) their state ids.
+                const uint32_t ncl = T.ncodes[l];
+                const uint32_t c0 = T.code[l][0];
+                const uint32_t pc1 = ncl == 2 ? T.code[l][1] : lnext != 0xffffffffu ? T.code[lnext][0] : c0;
+                const uint32_t ml_l = T.ml_off[l];
+                const uint32_t nn = lnext != 0xffffffffu ? T.n_delta[lnext] : 0u;      // lnext's entries, offsets
+                const uint32_t eo_n = lnext != 0xffffffffu ? T.ent_off[lnext] : 0u, mo_n = lnext != 0xffffffffu ? T.ml_off[lnext] : 0u;
+                const int tb_l = st == 0 ? lb : 3 - lb;
+                uint32_t plan = 1u | (2u << 4);      // n_out | sel << 2 of the single shape, and of the pair shape << 4
+                float thr_s0 = 0.f, thr_p0 = 0.f, thr_p1 = 0.f, base_thr_l = 0.f;
+                uint32_t sids = 0xffffffu;           // state ids of the out codes, one byte each: single, pair 0, pair 1;
+                                                     // byte 3 bit 0 / 1: the single / pair ids are looked up
+                if (MODE == MODE_PILEUP && (FAST_ONLY || fast_read)) {
+                    uint32_t ps = 1, pp = 2;
+                    if (c_par.numeric_mode == 2) {
+                        const uint32_t drop = c_par.collapse_code;
+                        if (c0 == drop) ps = 0;
+                        pp = c0 == drop ? (1u | 4u) : pc1 == drop ? 1u : 2u;
+                    }
+                    if (pp == 2 && (bucket4(c0) != bucket4(pc1) ? (bucket4(pc1) < bucket4(c0)) : (bucket4(c0) == 3))) pp |= 4u;
+                    plan = ps | (pp << 4);
+                    base_thr_l = c_par.base_set[tb_l] ? c_par.base_thr[tb_l] : c_par.default_thr;
+                    thr_s0 = mod_threshold(c0, tb_l, base_thr_l);
+                    thr_p0 = mod_threshold((pp & 4u) ? pc1 : c0, tb_l, base_thr_l);
+                    thr_p1 = mod_threshold((pp & 4u) ? c0 : pc1, tb_l, base_thr_l);
+                }
                 for (uint32_t j0 = 0; j0 < n; j0 += 32) {
                     uint32_t j = j0 + lane;
                     bool active = j < n;
@@ -1119,6 +1202,15 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                     uint32_t hist_q = 0;
                     if (active) {
                         uint32_t f = Pl[j];
+                        // register-only path: the entry's ML byte(s) and lnext's entry at the same index do not depend on f;
+                        // loaded beside it, the loads overlap instead of each waiting on the one before
+                        uint32_t ma = 0, mb = 0, p2j = 0xffffffffu, qn = 0;
+                        if (FAST_ONLY || fast_read) {
+                            const uint8_t* mlq = ml + ml_l + (size_t)j * ncl;
+                            ma = mlq[0];
+                            if (ncl == 2) mb = mlq[1];
+                            if (j < nn) { p2j = P[eo_n + j]; qn = ml[mo_n + j]; }
+                        }
                         uint32_t q = rev ? L - 1u - f : f;
                         // forward-read base at f: the list's own base (the position was selected as one of its occurrences);
                         // only 'N' lists have to look at the sequence (mod_bam.rs:1245)
@@ -1152,83 +1244,80 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                             uint32_t k = lower_bound_u32(P2, n2, f);
                             if (k < n2 && P2[k] == f) owner = false;
                         }
+                        RCLK_MARK;
                         if (owner && !e2) {
                             const int tb = st == 0 ? b : 3 - b;
                             uint32_t mask = 0, ccode = 0;      // observed states, called code
+                            uint32_t csid = 0;                 // state id of the called code (register-only pileup path)
                             int kind = 0;                      // 0 filtered, 1 canonical, 2 modified
                             float hv = 0.f;                    // arg-max value (histogram mode)
                             if (FAST_ONLY || fast_read) {
                                 // ---- register-only path: at most two codes at the position (one list with <= 2 codes, or
                                 //      two single-code lists of the strand). Same arithmetic as the generic path below.
-                                uint32_t c0 = T.code[l][0], c1 = 0;
                                 float p0, p1 = 0.f;
-                                int n2c = 1;
+                                bool pair = false;
                                 {
-                                    const uint8_t* mlq = ml + T.ml_off[l] + (size_t)j * T.ncodes[l];
-                                    p0 = __fdiv_rn(__fadd_rn((float)mlq[0], 0.5f), 256.0f);
-                                    if (T.ncodes[l] == 2) {
-                                        const float pb = __fdiv_rn(__fadd_rn((float)mlq[1], 0.5f), 256.0f);
-                                        const uint32_t cb = T.code[l][1];
-                                        if (cb == c0) { if (__fadd_rn(p0, pb) > 1.01f) e2 = true; else p0 = __fadd_rn(p0, pb); }
-                                        else { c1 = cb; p1 = pb; n2c = 2; }
+                                    p0 = ml_prob(ma);
+                                    if (ncl == 2) {
+                                        const float pb = ml_prob(mb);
+                                        if (pc1 == c0) { if (__fadd_rn(p0, pb) > 1.01f) e2 = true; else p0 = __fadd_rn(p0, pb); }
+                                        else { p1 = pb; pair = true; }
                                     }
                                 }
                                 if (lnext != 0xffffffffu && !e2) {       // the strand's other list (single code by construction)
-                                    const uint32_t* P2 = P + T.ent_off[lnext];
-                                    const uint32_t nn = T.n_delta[lnext];
+                                    const uint32_t* P2 = P + eo_n;
                                     uint32_t k = j;
-                                    const uint8_t* mln = ml + T.ml_off[lnext];
-                                    const uint32_t p2j = j < nn ? P2[j] : 0xffffffffu;
-                                    uint8_t qn = j < nn ? mln[j] : 0;          // same index in the other list: the usual case
-                                    bool found = j < nn && p2j == f;
+                                    const uint8_t* mln = ml + mo_n;
+                                    bool found = j < nn && p2j == f;          // same index in the other list: the usual case
                                     if (found) matched_next = true;
                                     else { k = lower_bound_u32(P2, nn, f); found = k < nn && P2[k] == f; if (found) qn = mln[k]; }
                                     if (found) {
-                                        const float pn = __fdiv_rn(__fadd_rn((float)qn, 0.5f), 256.0f);
-                                        const uint32_t cn = T.code[lnext][0];
-                                        if (cn == c0) p0 = __fadd_rn(p0, pn);
-                                        else { c1 = cn; p1 = pn; n2c = 2; }
-                                        if ((n2c == 2 ? __fadd_rn(p0, p1) : p0) > 1.01f) e2 = true;   // combine_checked
+                                        const float pn = ml_prob(qn);
+                                        if (pc1 == c0) p0 = __fadd_rn(p0, pn);
+                                        else { p1 = pn; pair = true; }
+                                        if ((pair ? __fadd_rn(p0, p1) : p0) > 1.01f) e2 = true;   // combine_checked
                                     }
                                 }
                                 if (!e2) {
-                                    if (c_par.numeric_mode == 2) {       // ReDistribute (mod_bam.rs:558-600)
-                                        const uint32_t drop = c_par.collapse_code;
-                                        if (n2c == 1) {
-                                            if (c0 == drop) n2c = 0;
-                                            else p0 = __fadd_rn(p0, __fdiv_rn(0.f, 2.0f));
-                                        } else if (c0 == drop) { c0 = c1; p0 = __fadd_rn(p1, __fdiv_rn(p0, 2.0f)); n2c = 1; }
-                                        else if (c1 == drop) { p0 = __fadd_rn(p0, __fdiv_rn(p1, 2.0f)); n2c = 1; }
-                                        else { const float sh = __fdiv_rn(0.f, 3.0f); p0 = __fadd_rn(p0, sh); p1 = __fadd_rn(p1, sh); }
-                                    }
-                                    // FxHashMap iteration order of the (<= 2) codes
-                                    if (n2c == 2) {
-                                        const uint32_t b0 = bucket4(c0), b1 = bucket4(c1);
-                                        if (b0 != b1 ? (b1 < b0) : (b0 == 3)) { const uint32_t tc = c0; c0 = c1; c1 = tc; const float tp = p0; p0 = p1; p1 = tp; }
-                                    }
-                                    const float sum = n2c == 0 ? 0.f : n2c == 1 ? __fadd_rn(0.f, p0) : __fadd_rn(__fadd_rn(0.f, p0), p1);
-                                    const float cp = __fsub_rn(1.0f, sum);
                                     if (MODE == MODE_PILEUP) {
-                                        if (n2c >= 1) mask |= 1u << state_id(C, scache, tb, c0);
-                                        if (n2c == 2) mask |= 1u << state_id(C, scache, tb, c1);
-                                        const float base_thr = c_par.base_set[tb] ? c_par.base_thr[tb] : c_par.default_thr;
+                                        // the list's plan for the entry's shape: ReDistribute, FxHash order, thresholds
+                                        const uint32_t pw = pair ? plan >> 4 : plan;
+                                        const uint32_t n_out = pw & 3u;
+                                        const bool sel = pw & 4u;
+                                        float o0 = sel ? p1 : p0;
+                                        const float o1 = sel ? p0 : p1;
+                                        if (n_out == 1) o0 = __fadd_rn(o0, half_share(o1));     // single: p1 == 0 adds nothing
+                                        const float sum = n_out == 0 ? 0.f : n_out == 1 ? o0 : __fadd_rn(o0, o1);
+                                        const float cp = __fsub_rn(1.0f, sum);
                                         bool have = false;
                                         float best = 0.f;
-                                        for (int k2 = 0; k2 < n2c; k2++) {
-                                            const uint32_t cc = k2 == 0 ? c0 : c1;
-                                            const float pp = k2 == 0 ? p0 : p1;
-                                            float thr = base_thr;
-                                            if (c_par.n_mod_thr) {
-                                                const uint32_t any_code = (uint32_t)("ACGT"[tb]);
-                                                bool fnd = false;
-                                                for (uint32_t t = 0; t < c_par.n_mod_thr && !fnd; t++) if (c_par.mod_code[t] == cc) { thr = c_par.mod_thr[t]; fnd = true; }
-                                                for (uint32_t t = 0; t < c_par.n_mod_thr && !fnd; t++) if (c_par.mod_code[t] == any_code) { thr = c_par.mod_thr[t]; fnd = true; }
-                                            }
-                                            if (pp >= thr && (!have || pp >= best)) { have = true; best = pp; kind = 2; ccode = cc; }
-                                        }
-                                        if (cp >= base_thr && (!have || cp >= best)) { have = true; kind = 1; }
+                                        uint32_t called = 0;
+                                        if (n_out >= 1 && o0 >= (pair ? thr_p0 : thr_s0)) { have = true; best = o0; kind = 2; }
+                                        if (n_out == 2 && o1 >= thr_p1 && (!have || o1 >= best)) { have = true; best = o1; kind = 2; called = 1; }
+                                        if (cp >= base_thr_l && (!have || cp >= best)) { have = true; kind = 1; }
                                         if (!have) kind = 0;
+                                        // state ids: registered when a lane first meets the shape, as every entry would
+                                        if (n_out != 0) {
+                                            const uint32_t sh = pair ? 8u : 0u;
+                                            if (!((sids >> (24u + (sh >> 3))) & 1u)) {
+                                                const uint32_t s0 = (uint32_t)state_id(C, scache, tb_l, sel ? pc1 : c0);
+                                                sids = (sids & ~(0xffu << sh)) | (s0 << sh) | (1u << (24u + (sh >> 3)));
+                                                if (n_out == 2) sids = (sids & 0xff00ffffu) | ((uint32_t)state_id(C, scache, tb_l, sel ? c0 : pc1) << 16);
+                                            }
+                                            mask = (1u << ((sids >> sh) & 0xffu)) | (n_out == 2 ? 1u << ((sids >> 16) & 0xffu) : 0u);
+                                            csid = (sids >> (sh + 8u * called)) & 0xffu;
+                                        }
                                     } else {
+                                        uint32_t k0 = c0, k1 = pair ? pc1 : 0u;
+                                        int n2c = pair ? 2 : 1;
+                                        if (c_par.numeric_mode == 2) redistribute2(c_par.collapse_code, k0, p0, k1, p1, n2c);
+                                        // FxHashMap iteration order of the (<= 2) codes
+                                        if (n2c == 2) {
+                                            const uint32_t b0 = bucket4(k0), b1 = bucket4(k1);
+                                            if (b0 != b1 ? (b1 < b0) : (b0 == 3)) { const uint32_t tc = k0; k0 = k1; k1 = tc; const float tp = p0; p0 = p1; p1 = tp; }
+                                        }
+                                        const float sum = n2c == 0 ? 0.f : n2c == 1 ? __fadd_rn(0.f, p0) : __fadd_rn(__fadd_rn(0.f, p0), p1);
+                                        const float cp = __fsub_rn(1.0f, sum);
                                         float mp = 0.f;
                                         bool hm2 = false;
                                         if (n2c >= 1) { mp = p0; hm2 = true; }
@@ -1237,22 +1326,15 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                                         if (C.summ || C.qhist) {
                                             // thresholded call (as in the pileup) and arg-max call (last maximum wins, mod_bam.rs:489-505)
                                             uint32_t s0 = 0, s1 = 0;
-                                            if (n2c >= 1) { s0 = (uint32_t)state_id(C, scache, tb, c0); mask |= 1u << s0; }
-                                            if (n2c == 2) { s1 = (uint32_t)state_id(C, scache, tb, c1); mask |= 1u << s1; }
+                                            if (n2c >= 1) { s0 = (uint32_t)state_id(C, scache, tb, k0); mask |= 1u << s0; }
+                                            if (n2c == 2) { s1 = (uint32_t)state_id(C, scache, tb, k1); mask |= 1u << s1; }
                                             const float base_thr = c_par.base_set[tb] ? c_par.base_thr[tb] : c_par.default_thr;
                                             bool have = false;
                                             float best = 0.f;
                                             uint32_t tk = 0, ts = 0;
                                             for (int k2 = 0; k2 < n2c; k2++) {
-                                                const uint32_t cc = k2 == 0 ? c0 : c1;
                                                 const float pp = k2 == 0 ? p0 : p1;
-                                                float thr = base_thr;
-                                                if (c_par.n_mod_thr) {
-                                                    const uint32_t any_code = (uint32_t)("ACGT"[tb]);
-                                                    bool fnd = false;
-                                                    for (uint32_t t = 0; t < c_par.n_mod_thr && !fnd; t++) if (c_par.mod_code[t] == cc) { thr = c_par.mod_thr[t]; fnd = true; }
-                                                    for (uint32_t t = 0; t < c_par.n_mod_thr && !fnd; t++) if (c_par.mod_code[t] == any_code) { thr = c_par.mod_thr[t]; fnd = true; }
-                                                }
+                                                const float thr = mod_threshold(k2 == 0 ? k0 : k1, tb, base_thr);
                                                 if (pp >= thr && (!have || pp >= best)) { have = true; best = pp; tk = 2; ts = k2 == 0 ? s0 : s1; }
                                             }
                                             if (cp >= base_thr && (!have || cp >= best)) { have = true; tk = 1; }
@@ -1269,7 +1351,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                             int ord[MAX_MAP];
                             const uint8_t* mlq = ml + T.ml_off[l] + (size_t)j * T.ncodes[l];
                             for (uint32_t c = 0; c < T.ncodes[l] && !e2; c++) {
-                                const float p = __fdiv_rn(__fadd_rn((float)mlq[c], 0.5f), 256.0f);
+                                const float p = ml_prob(mlq[c]);
                                 const int it = m.find(T.code[l][c]);
                                 if (it < 0) { if (!m.push(T.code[l][c], p)) { atomicOr(C.err, MKP_DERR_TOO_MANY_CODES); e2 = true; } }
                                 else { if (__fadd_rn(m.p[it], p) > 1.01f) e2 = true; else m.p[it] = __fadd_rn(m.p[it], p); }
@@ -1286,7 +1368,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                                 t2.n = 0;
                                 const uint8_t* ml2 = ml + T.ml_off[l2] + (size_t)k * T.ncodes[l2];
                                 for (uint32_t c = 0; c < T.ncodes[l2] && !e2; c++) {
-                                    const float p = __fdiv_rn(__fadd_rn((float)ml2[c], 0.5f), 256.0f);
+                                    const float p = ml_prob(ml2[c]);
                                     const int it = t2.find(T.code[l2][c]);
                                     if (it < 0) { if (!t2.push(T.code[l2][c], p)) { atomicOr(C.err, MKP_DERR_TOO_MANY_CODES); e2 = true; } }
                                     else { if (__fadd_rn(t2.p[it], p) > 1.01f) e2 = true; else t2.p[it] = __fadd_rn(t2.p[it], p); }
@@ -1332,6 +1414,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                                 }
                             }
                             }
+                            RCLK_MARK;
                             if (!e2) {
                                 bool keep = trim_ok;
                                 if (keep && c_par.edge_on) {
@@ -1356,7 +1439,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                                         // positions outside the focus set (motif / include-bed) are dropped when the hot bitmap
                                         // is ranked (k_block_popc) and skipped by k_count_calls: no bitmap lookup here
                                         if (aligned && rpos >= C.cs && rpos < C.ce) {
-                                            const uint32_t state = kind == 0 ? 0u : kind == 1 ? 1u : 2u + (uint32_t)state_id(C, scache, tb, ccode);
+                                            const uint32_t state = kind == 0 ? 0u : kind == 1 ? 1u : 2u + ((FAST_ONLY || fast_read) ? csid : (uint32_t)state_id(C, scache, tb, ccode));
                                             // does a '+' list cover the same position (both pos_call and neg_call present)?
                                             uint32_t nosub = 0;
                                             if (st == 1) {
@@ -1420,11 +1503,13 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                         }
                         n_hist += __popc(hm);
                     }
+                    RCLK_ROUND;
                 }
                 if (n_calls != calls_before) n_runs++;
                 if (!imp_any && lnext != 0xffffffffu && T.base[lnext] != 'N' && T.n_delta[lnext] == cnt_next) skip_mask |= 1u << lnext;
             }
         }
+        RCLK(3);
         // ---- phase 4b: implicit tables (every other occurrence of the base is an inferred-canonical entry) ----
         uint32_t imp_meta[2] = {0, 0};
         unsigned long long imp_hist[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -1604,7 +1689,10 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
         }
         if (lane == 0) C.meta[ri] = meta;
         __syncwarp();
+        RCLK(5);
     }
+    RCLK(0);
+    RCLK_FLUSH;
 }
 
 // ---- rank over the hot bitmap -----------------------------------------------------------------------
