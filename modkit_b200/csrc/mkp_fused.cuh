@@ -108,11 +108,6 @@ __device__ __forceinline__ int state_id_fz(const FusedDev& F, StateCache& sc, in
     return id;
 }
 
-__device__ __forceinline__ bool edge_keep(uint32_t f, uint32_t L) {
-    if (!c_par.edge_on) return true;
-    return c_par.edge_inv ? (f < c_par.edge_start || f >= L - c_par.edge_end) : (f >= c_par.edge_start && f < L - c_par.edge_end);
-}
-
 // one read, one warp
 // MM list discovery (src/mod_bam.rs:900-1000), shape classification and tokens -> occurrence indices (src/mod_bam.rs:667-767) of one
 // read by one warp. P receives the 0-based occurrence index of every token (per list at T.ent_off[l]); `slow` = the read goes to

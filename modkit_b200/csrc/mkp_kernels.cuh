@@ -1,19 +1,22 @@
-// Device kernels of the H100-native `modkit pileup` hot path (sm_90a).
+// Device kernels of the H100-native `modkit pileup` hot path (sm_90a), and of pileup-hemi, threshold estimation, `summary` and
+// `sample-probs` over the same decode. DESIGN §4.1 describes the pass.
 //
-// Pipeline per chunk (all on one stream, intermediates stay in L2/HBM):
-//   k_decode      warp per read: CIGAR prefix, MM text parse, delta -> forward position (rank/select on
-//                 the 4-bit SEQ), ML -> probability, list merging, collapse, threshold call, projection
-//                 to reference coordinates; emits compact call records + marks the hot-position bitmap.
-//                 (reference: src/mod_bam.rs:900-1577, src/read_cache.rs:69-211,
-//                  src/threshold_mod_caller.rs:28-63, src/util.rs:122-145)
-//   k_rank_*      popcount prefix over the hot bitmap  -> counter slot index per hot position
-//   k_count_calls one thread per call record: modcall / filtered counters (src/pileup/mod.rs:876-937)
-//   k_count_bases warp per read: walks CIGAR + SEQ with bit-parallel window tests against the hot
-//                 bitmap; base / delete counters and observed-code masks (src/pileup/mod.rs:831-874)
-//   k_rows_*      per slot: FeatureVector::decode (src/pileup/mod.rs:283-445) -> mkp_row
-//   k_hemi_count, k_hemi_rows   `pileup-hemi` over the same decode: duplex pattern counters per + strand motif position and
+// Per chunk, on one stream (intermediates stay in L2/HBM):
+//   k_parse       warp per read: admission, reference span, MM list discovery and delta parse, rank/select on the 4-bit SEQ
+//                 -> forward position of every list entry, ML length checks, implicit-mode bookkeeping; hands a list table to
+//                 k_resolve (src/mod_bam.rs:900-1000, 667-767, 1213-1295, src/read_cache.rs:122-137)
+//   k_resolve     warp per read, lane per list entry: CIGAR prefix, list merging, collapse, threshold call (MODE_PILEUP) or
+//                 histogram / summary value (MODE_HIST), edge filter, projection to reference coordinates; emits call records,
+//                 observed-code masks, implicit tables and hot-bitmap marks (src/mod_bam.rs:530-656, src/read_cache.rs:69-211,
+//                 src/threshold_mod_caller.rs:28-63, src/util.rs:122-145, src/summarize.rs:117-252)
+//   k_block_popc, k_scan_blocks, k_word_prefix, k_word_record   rank over the hot bitmap -> counter slot per hot position
+//   k_count_calls warp per read, lanes over its call records: modcall / canonical / filtered counters (src/pileup/mod.rs:876-937)
+//   k_count_bases warp per work item (a window of a read's reference span): base / delete counters under the hot positions and
+//                 observed-code masks; counts the call records of reads with one sorted run itself (src/pileup/mod.rs:831-874)
+//   k_rows        thread per bitmap word: FeatureVector::decode (src/pileup/mod.rs:283-445) -> mkp_row
+//   k_hemi_count, k_hemi_rows   `pileup-hemi`: duplex pattern counters per + strand motif position and
 //                 DuplexFeatureVector::decode -> mkp_hemi_row (src/pileup/duplex.rs)
-// Integer/indexing work: no tensor cores; the bound is HBM bandwidth.
+// Integer and indexing work: no tensor cores, and far from bound by HBM bandwidth (DESIGN §11).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -53,7 +56,7 @@ struct DevParams {
     uint32_t edge_on, edge_inv, edge_start, edge_end;
 };
 
-struct ReadMeta {       // 40 bytes, written by k_decode
+struct ReadMeta {       // 40 bytes, written by k_parse and k_resolve
     int32_t ref_end;
     uint32_t flags;     // bit0 admitted, bit1 has mod info (not in skip_set), bit2 call records are one position-sorted run
     uint32_t pos_mask, neg_mask;
@@ -116,6 +119,48 @@ struct ChunkDev {
 __constant__ DevParams c_par;
 
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
+
+// --edge-filter (src/util.rs:122-145): a read no longer than either edge has no position the filter keeps
+__device__ __forceinline__ bool edge_read_ok(uint32_t L) { return !c_par.edge_on || !(L <= c_par.edge_start || L <= c_par.edge_end); }
+// does forward position f of a read of length L pass the filter? Only for a read that passes edge_read_ok (L > edge_end).
+// k_count_bases and k_hemi_count call it without that guard: k_resolve gives no such read an implicit table
+__device__ __forceinline__ bool edge_keep(uint32_t f, uint32_t L) {
+    bool keep = true;
+    if (c_par.edge_on) {
+        if (c_par.edge_inv) keep = f < c_par.edge_start || f >= L - c_par.edge_end;
+        else keep = f >= c_par.edge_start && f < L - c_par.edge_end;
+    }
+    return keep;
+}
+// threshold of canonical base tb: its --filter-threshold, else the default one
+__device__ __forceinline__ float base_threshold(int tb) { return c_par.base_set[tb] ? c_par.base_thr[tb] : c_par.default_thr; }
+
+// CIGAR op classes: query length, reference length, and M/=/X (a base aligned to the reference)
+__device__ __forceinline__ bool cig_is_match(uint32_t op) { return op == 0 || op == 7 || op == 8; }
+__device__ __forceinline__ uint32_t cig_qlen(uint32_t op, uint32_t len) { return (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) ? len : 0u; }
+__device__ __forceinline__ uint32_t cig_rlen(uint32_t op, uint32_t len) { return (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) ? len : 0u; }
+
+// MODE_PILEUP call record (reference position, info): info = mod strand | forward base << 1 | state << 3 | nosub << 11, with
+// state 0 filtered, 1 canonical, 2 + id modified, and nosub set on a '-' record whose position a '+' list also holds
+__device__ __forceinline__ uint32_t call_info(uint32_t st, uint32_t b, uint32_t state, uint32_t nosub) { return st | (b << 1) | (state << 3) | (nosub << 11); }
+__device__ __forceinline__ uint32_t call_strand(uint32_t info) { return info & 1u; }
+__device__ __forceinline__ uint32_t call_base(uint32_t info) { return (info >> 1) & 3u; }
+__device__ __forceinline__ uint32_t call_state(uint32_t info) { return (info >> 3) & 0xffu; }
+__device__ __forceinline__ uint32_t call_nosub(uint32_t info) { return (info >> 11) & 1u; }
+
+// MODE_HIST value record (key, value): key = bin | canonical base << 16 | inexact << 20 | qual << 21. With summ / qhist the
+// value is the classification: thresholded kind | its state id << 2 | arg-max kind << 8 | its state id << 10 (kind 0 filtered,
+// 1 canonical, 2 modified; a state id is only read with kind 2)
+__device__ __forceinline__ uint32_t sample_key(uint32_t bin, uint32_t base, uint32_t inexact, uint32_t qual) { return bin | (base << 16) | (inexact << 20) | (qual << 21); }
+__device__ __forceinline__ uint32_t sample_bin(uint32_t key) { return key & 0xffffu; }
+__device__ __forceinline__ uint32_t sample_base(uint32_t key) { return (key >> 16) & 3u; }
+__device__ __forceinline__ uint32_t sample_inexact(uint32_t key) { return (key >> 20) & 1u; }
+__device__ __forceinline__ uint32_t sample_qual(uint32_t key) { return (key >> 21) & 255u; }
+__device__ __forceinline__ uint32_t sample_class(uint32_t tk, uint32_t ts, uint32_t ak, uint32_t as) { return tk | (ts << 2) | (ak << 8) | (as << 10); }
+__device__ __forceinline__ uint32_t class_tkind(uint32_t c) { return c & 3u; }
+__device__ __forceinline__ uint32_t class_tstate(uint32_t c) { return (c >> 2) & 63u; }
+__device__ __forceinline__ uint32_t class_akind(uint32_t c) { return (c >> 8) & 3u; }
+__device__ __forceinline__ uint32_t class_astate(uint32_t c) { return (c >> 10) & 63u; }
 
 // prob_to_qual (mod_bam.rs:798-806): exactly 1.0 -> 255, else floor(p * 256) in f32 with Rust's saturating `as u8` (NaN and
 // negatives -> 0, values from 255/256 up -> 255)
@@ -181,7 +226,6 @@ struct ProbMap {
         while (slot[s] >= 0) s = (s + 1) & (nb - 1);
         slot[s] = (int8_t)item;
     }
-    __device__ int find(uint32_t c) const { for (int i = 0; i < n; i++) if (code[i] == c) return i; return -1; }
     // returns item index, or -1 on overflow
     __device__ __noinline__ int insert(uint32_t c, float v) {
         if (n >= MAX_MAP) return -1;
@@ -196,59 +240,7 @@ struct ProbMap {
         place(n);
         return n++;
     }
-    // item at iteration rank k (k < n)
-    __device__ int item_at(int k) const {
-        for (int s = 0; s < 8; s++) if (slot[s] >= 0) { if (k == 0) return slot[s]; k--; }
-        return -1;
-    }
-    __device__ float sum() const {
-        float s = 0.f;
-        for (int k = 0; k < 8; k++) if (slot[k] >= 0) s = __fadd_rn(s, p[slot[k]]);
-        return s;
-    }
 };
-
-// CollapseMethod::ReDistribute (src/mod_bam.rs:558-600)
-__device__ __noinline__ void redistribute(const ProbMap& in, uint32_t drop, ProbMap& out) {
-    float marginal = 0.f;
-    int n_other = 0;
-    for (int s = 0; s < 8; s++) if (in.slot[s] >= 0) { int it = in.slot[s]; if (in.code[it] == drop) marginal = __fadd_rn(marginal, in.p[it]); else n_other++; }
-    float share = __fdiv_rn(marginal, __fadd_rn((float)n_other, 1.0f));
-    out.init();
-    for (int s = 0; s < 8; s++) if (in.slot[s] >= 0) { int it = in.slot[s]; if (in.code[it] != drop) out.insert(in.code[it], __fadd_rn(in.p[it], share)); }
-}
-
-// MultipleThresholdModCaller::call (src/threshold_mod_caller.rs:28-63): 0 filtered, 1 canonical, 2 = modified (code in *code)
-__device__ __noinline__ int make_call(const ProbMap& m, int tb, uint32_t* code) {
-    bool have = false;
-    float best = 0.f;
-    int kind = 0;
-    const uint32_t any_code = (uint32_t)("ACGT"[tb]);
-    for (int s = 0; s < 8; s++) {
-        if (m.slot[s] < 0) continue;
-        int it = m.slot[s];
-        uint32_t c = m.code[it];
-        float thr;
-        bool found = false;
-        for (uint32_t k = 0; k < c_par.n_mod_thr && !found; k++) if (c_par.mod_code[k] == c) { thr = c_par.mod_thr[k]; found = true; }
-        for (uint32_t k = 0; k < c_par.n_mod_thr && !found; k++) if (c_par.mod_code[k] == any_code) { thr = c_par.mod_thr[k]; found = true; }
-        if (!found) thr = c_par.base_set[tb] ? c_par.base_thr[tb] : c_par.default_thr;
-        float pm = m.p[it];
-        if (pm >= thr) { if (!have || pm >= best) { have = true; best = pm; kind = 2; *code = c; } }
-    }
-    float cthr = c_par.base_set[tb] ? c_par.base_thr[tb] : c_par.default_thr;
-    float cp = __fsub_rn(1.0f, m.sum());
-    if (cp >= cthr) { if (!have || cp >= best) { have = true; best = cp; kind = 1; } }
-    return have ? kind : 0;
-}
-// BaseModProbs::argmax_base_mod_call value (src/mod_bam.rs:489-505)
-__device__ __noinline__ float argmax_prob(const ProbMap& m) {
-    float cp = __fsub_rn(1.0f, m.sum());
-    bool have = false;
-    float mp = 0.f;
-    for (int s = 0; s < 8; s++) if (m.slot[s] >= 0) { float v = m.p[m.slot[s]]; if (!have || v >= mp) { have = true; mp = v; } }
-    return (have && mp > cp) ? mp : cp;
-}
 
 // ---- probabilities of one read position in insertion order (BaseModProbs) ---------------------------------------
 struct Items {
@@ -320,7 +312,7 @@ __device__ __forceinline__ int make_call_items(const Items& it, const int* ord, 
     bool have = false;
     float best = 0.f;
     int kind = 0;
-    const float base_thr = c_par.base_set[tb] ? c_par.base_thr[tb] : c_par.default_thr;
+    const float base_thr = base_threshold(tb);
     for (int k = 0; k < it.n; k++) {
         const int i = ord[k];
         const uint32_t c = it.code[i];
@@ -332,6 +324,7 @@ __device__ __forceinline__ int make_call_items(const Items& it, const int* ord, 
     if (cp >= base_thr && (!have || cp >= best)) { have = true; kind = 1; }
     return have ? kind : 0;
 }
+
 // BaseModProbs::argmax_base_mod_call value (src/mod_bam.rs:489-505)
 __device__ __forceinline__ float argmax_items(const Items& it, const int* ord) {
     const float cp = __fsub_rn(1.0f, items_sum(it, ord));
@@ -519,8 +512,8 @@ __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
             uint32_t rsum = 0;
 #pragma unroll 4
             for (uint32_t i = lane; i < h.n_cigar; i += 32) {
-                const uint32_t c = cig[i], op = c & 15;
-                if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) rsum += c >> 4;
+                const uint32_t c = cig[i];
+                rsum += cig_rlen(c & 15, c >> 4);
             }
             meta.ref_end = (int32_t)((uint32_t)h.ref_start + __reduce_add_sync(FULL, rsum));
         }
@@ -999,6 +992,197 @@ __global__ void __launch_bounds__(128, MKP_MINB_PARSE) k_parse(ChunkDev C) {
     PCLK_FLUSH;
 }
 
+// canonical base of implicit table sb (mod strand sb >> 2, forward base sb & 3)
+__device__ __forceinline__ int table_base(int sb) { return (sb >> 2) == 0 ? (sb & 3) : 3 - (sb & 3); }
+
+// the read's list table, handed over by k_parse, into the warp's shared copy
+__device__ __forceinline__ void load_list_table(ListTab& T, const ReadLists* R, uint32_t nl, uint32_t lane) {
+    __syncwarp();
+    if (lane < nl) {
+        const ListRec rec = R->rec[lane];
+        T.n_delta[lane] = rec.n_delta; T.ent_off[lane] = rec.ent_off; T.ml_off[lane] = rec.ml_off;
+        for (int c = 0; c < MAX_LIST_CODES; c++) T.code[lane][c] = rec.code[c];
+        T.base[lane] = rec.base; T.strand[lane] = rec.strand; T.mode[lane] = rec.mode; T.ncodes[lane] = rec.ncodes;
+    }
+    __syncwarp();
+}
+
+// register-only path: no implicit tables, no 'N' list, and per strand either one list with <= 2 codes or two single-code lists
+__device__ __forceinline__ bool fast_shape(const ListTab& T, uint32_t nl, bool imp_any) {
+    bool fast = !imp_any;
+    uint32_t cnt0 = 0, cnt1 = 0, max0 = 0, max1 = 0;
+    for (uint32_t l2 = 0; l2 < nl; l2++) {
+        if (T.base[l2] == 'N') fast = false;
+        if (!T.n_delta[l2]) continue;
+        const uint32_t ncd = T.ncodes[l2];
+        if (T.strand[l2]) { cnt1++; max1 = max(max1, ncd); } else { cnt0++; max0 = max(max0, ncd); }
+    }
+    if (!(cnt0 <= 1 ? max0 <= 2 : (cnt0 == 2 && max0 == 1))) fast = false;
+    if (!(cnt1 <= 1 ? max1 <= 2 : (cnt1 == 2 && max1 == 1))) fast = false;
+    return fast;
+}
+
+// query position -> reference position over the read's CIGAR prefix: cq[i] = 2 * query start of op i + (op i is M/=/X), one
+// sentinel cq[nc] = 2 * query length; cr[i] = reference start of op i; qt[t] = the op that holds query base t << qt_shift
+struct QueryMap {
+    uint32_t* cq;
+    uint32_t* cr;
+    uint16_t* qt;
+    uint32_t nc, q_total, qt_shift;
+    bool use_qt;
+};
+
+// CIGAR prefix: query / reference start of every op; four ops per lane (one 16-byte load), 128 per round
+__device__ __forceinline__ void cigar_prefix(QueryMap& M, const uint32_t* cig, uint32_t ref_start, uint32_t lane) {
+    const uint32_t nc = M.nc;
+    uint32_t qc = 0, rc = ref_start;
+    for (uint32_t b = 0; b < nc; b += 128) {
+        const uint32_t i = b + 4 * lane;
+        uint4 c4 = make_uint4(0, 0, 0, 0);
+        if (i < nc) c4 = *(const uint4*)(cig + i);    // 16-byte aligned; words past nc belong to the read's own block
+        const uint32_t cw[4] = {c4.x, c4.y, c4.z, c4.w};
+        uint32_t ql[4], rl[4], qs = 0, rs = 0;
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const uint32_t c = i + k < nc ? cw[k] : 0u, op = c & 15, len = c >> 4;
+            // (spelled out: through cig_qlen / cig_rlen nvcc evaluates the classes with 16 more instructions in this loop)
+            ql[k] = (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) ? len : 0;
+            rl[k] = (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) ? len : 0;
+            qs += ql[k]; rs += rl[k];
+        }
+        const uint32_t qi = warp_incl_scan(qs), rr = warp_incl_scan(rs);
+        uint32_t q0 = qc + qi - qs, r0 = rc + rr - rs;
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            if (i + k < nc) {
+                const uint32_t op = cw[k] & 15;
+                M.cq[i + k] = 2u * q0 + (cig_is_match(op) ? 1u : 0u);
+                M.cr[i + k] = r0;
+            }
+            q0 += ql[k]; r0 += rl[k];
+        }
+        qc += __shfl_sync(FULL, qi, 31);
+        rc += __shfl_sync(FULL, rr, 31);
+    }
+    if (lane == 0) M.cq[nc] = 2u * qc;
+    M.q_total = qc;
+    __syncwarp();
+}
+
+// query -> op table: qt[t] = the op that holds query base t << shift (the largest i with cq[i] <= that base)
+__device__ __forceinline__ void query_op_table(QueryMap& M, uint32_t lane) {
+    const uint32_t nc = M.nc;
+    uint32_t qt_shift = 7;
+    while (qt_shift < 31 && (M.q_total >> qt_shift) >= (uint32_t)QT_CAP) qt_shift++;
+    M.qt_shift = qt_shift;
+    M.use_qt = nc > 0 && nc <= 65535u;
+    if (M.use_qt) {
+        const uint32_t B = 1u << qt_shift;
+        for (uint32_t i = lane; i < nc; i += 32) {
+            const uint32_t s0 = M.cq[i] >> 1, e0 = M.cq[i + 1] >> 1;
+            for (uint32_t m = (s0 + B - 1) & ~(B - 1); m < e0; m += B) M.qt[m >> qt_shift] = (uint16_t)i;
+        }
+        if (lane == 0) M.qt[(M.q_total + B - 1) >> qt_shift] = (uint16_t)(nc - 1);
+    }
+    __syncwarp();
+}
+
+// reference position of query position q, when an M/=/X op holds it: that op is the largest i with cq[i] >> 1 <= q, narrowed by
+// the table
+__device__ __forceinline__ bool project(const QueryMap& M, uint32_t q, uint32_t& rpos) {
+    bool aligned = false;
+    if (M.nc > 0 && q < M.q_total) {
+        uint32_t lo = 0, hi = M.nc;
+        if (M.use_qt) { const uint32_t t = q >> M.qt_shift; lo = M.qt[t]; hi = (uint32_t)M.qt[t + 1] + 1u; }
+        const uint32_t key = 2u * q + 1u;
+        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (M.cq[mid] <= key) lo = mid; else hi = mid; }
+        const uint32_t e = M.cq[lo];
+        if ((e & 1u) && q < (M.cq[lo + 1] >> 1)) { aligned = true; rpos = M.cr[lo] + (q - (e >> 1)); }
+    }
+    return aligned;
+}
+
+// Implicit tables ('.'/default mode, src/mod_bam.rs:1265-1292): every other occurrence of a table's base is an inferred-canonical
+// entry. A table survives the edge filter when some occurrence of its base keeps its forward position. MODE_PILEUP: the table's
+// call goes to imp_meta (ReadMeta::imp); MODE_HIST: imp_hist[sb] counts its inferred values that pass, explicit ones off.
+template <int MODE>
+__device__ __forceinline__ void implicit_tables(const ChunkDev& C, StateCache& scache, const ListTab& T, uint32_t nl, const uint32_t (*imp_lists)[4],
+                                                const mkp_read_hdr& h, const uint32_t* cig, const uint8_t* seq, uint32_t L, bool rev, uint32_t lane,
+                                                const uint32_t* imp_explicit, uint32_t* sum_obs, uint32_t& pos_mask, uint32_t& neg_mask,
+                                                bool& table_survived, uint32_t* imp_meta, unsigned long long* imp_hist) {
+    const bool trim_ok = edge_read_ok(L);
+    for (uint32_t sb = 0; sb < 8; sb++) {
+        const uint32_t s = sb >> 2, b = sb & 3;
+        const uint32_t lists = imp_lists[s][b];
+        if (!lists || !trim_ok) continue;
+        const uint32_t xn = 1u << (rev ? 3 - b : b);          // SEQ nibble of the forward base b
+        // survives the edge filter?  (any occurrence of the base with a kept forward position)
+        bool any = false;
+        for (uint32_t q = lane; q < L && !any; q += 32) {
+            if (seq_nibble(seq, q) != xn) continue;
+            const uint32_t f = rev ? L - 1u - q : q;
+            // (spelled out: through edge_keep, nvcc compiles this loop of k_resolve<MODE_HIST, false> to 296 more SASS lines)
+            bool keep = true;
+            if (c_par.edge_on) keep = c_par.edge_inv ? (f < c_par.edge_start || f >= L - c_par.edge_end) : (f >= c_par.edge_start && f < L - c_par.edge_end);
+            any = keep;
+        }
+        if (!__any_sync(FULL, any)) continue;
+        Items m, mc;
+        m.n = 0;
+        int ord[MAX_MAP];
+        for (uint32_t l = 0; l < nl; l++) if ((lists >> l) & 1u) for (uint32_t c = 0; c < T.ncodes[l]; c++) if (m.find(T.code[l][c]) < 0) m.push(T.code[l][c], 0.f);
+        iter_order(m, ord);
+        const Items* use = &m;
+        if (c_par.numeric_mode == 2) { redistribute_items(m, ord, c_par.collapse_code, mc); iter_order(mc, ord); use = &mc; }
+        const int tb = s == 0 ? (int)b : 3 - (int)b;
+        table_survived = true;
+        if (MODE == MODE_PILEUP) {
+            uint32_t mask = 0;
+            for (int k = 0; k < use->n; k++) mask |= 1u << state_id(C, scache, tb, use->code[k]);
+            if ((s == 0) != rev) pos_mask |= mask; else neg_mask |= mask;
+            uint32_t code = 0;
+            const int kind = make_call_items(*use, ord, tb, &code);
+            const uint32_t state = kind == 0 ? 0u : kind == 1 ? 1u : 2u + (uint32_t)state_id(C, scache, tb, code);
+            imp_meta[s] |= (0x80u | state) << (8 * b);
+        } else {
+            if (C.summ) for (int k = 0; k < use->n; k++) sum_obs[tb] |= 1u << state_id(C, scache, tb, use->code[k]);
+            // values: argmax of an all-zero map = canonical probability 1.0 for every passing inferred position
+            unsigned long long n_pass = 0;
+            if (C.hist_include_unaligned && !C.focus_pos) {
+                for (uint32_t q = lane; q < L; q += 32) {
+                    if (seq_nibble(seq, q) != xn) continue;
+                    const uint32_t f = rev ? L - 1u - q : q;
+                    if (edge_keep(f, L)) n_pass++;
+                }
+            } else {
+                uint32_t qc2 = 0, rc2 = (uint32_t)h.ref_start;
+                const uint32_t* bm = C.focus_pos ? (((s == 0) == rev) ? C.focus_neg : C.focus_pos) : nullptr;
+                for (uint32_t i = 0; i < h.n_cigar; i++) {
+                    const uint32_t c = cig[i], op = c & 15, len = c >> 4;
+                    if (cig_is_match(op)) {
+                        for (uint32_t k = lane; k < len; k += 32) {
+                            const uint32_t q = qc2 + k;
+                            if (q >= L || seq_nibble(seq, q) != xn) continue;
+                            const uint32_t f = rev ? L - 1u - q : q;
+                            bool keep = edge_keep(f, L);
+                            if (keep && bm) {
+                                const uint32_t r = rc2 + k;
+                                keep = r >= C.cs && r < C.ce && ((bm[(r - C.cs) >> 5] >> ((r - C.cs) & 31)) & 1u);
+                            }
+                            if (keep) n_pass++;
+                        }
+                    }
+                    qc2 += cig_qlen(op, len);
+                    rc2 += cig_rlen(op, len);
+                }
+            }
+            n_pass = __reduce_add_sync(FULL, (uint32_t)n_pass);
+            const uint32_t n_exp = __reduce_add_sync(FULL, imp_explicit[sb]);
+            imp_hist[sb] = n_pass > n_exp ? n_pass - n_exp : 0;
+        }
+    }
+}
+
 // Kernel B: per read with mod info: CIGAR prefix, then every list entry -> merged probabilities -> collapse ->
 // threshold call -> reference position; call records, observed-code masks, implicit tables, hot-bitmap marks.
 // FAST_ONLY = true: handles the reads whose lists fit the register-only path (no implicit tables, no 'N' list, at most
@@ -1043,97 +1227,28 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
         const uint32_t L = h.l_seq;
         const bool rev = h.flags & 0x10;
         const uint32_t* cig = (const uint32_t*)(C.heap + h.off);
-        uint32_t* const cq = h.n_cigar <= CQ_CAP ? s_cq[wib] : gcq;
-        uint32_t* const cr = h.n_cigar <= CQ_CAP ? s_cr[wib] : gcr;
-        uint16_t* const qt = s_qt[wib];
         const uint8_t* seq = C.heap + h.off + 4ull * h.n_cigar;
         const uint8_t* ml = seq + ((L + 1) >> 1);
         uint32_t imp_lists[2][4];
         for (int k = 0; k < 8; k++) imp_lists[k >> 2][k & 3] = R->imp_lists[k];
-        __syncwarp();
-        if (lane < nl) {
-            const ListRec rec = R->rec[lane];
-            T.n_delta[lane] = rec.n_delta; T.ent_off[lane] = rec.ent_off; T.ml_off[lane] = rec.ml_off;
-            for (int c = 0; c < MAX_LIST_CODES; c++) T.code[lane][c] = rec.code[c];
-            T.base[lane] = rec.base; T.strand[lane] = rec.strand; T.mode[lane] = rec.mode; T.ncodes[lane] = rec.ncodes;
-        }
-        __syncwarp();
+        load_list_table(T, R, nl, lane);
         bool imp_any = false;
         for (int k = 0; k < 8; k++) imp_any = imp_any || imp_lists[k >> 2][k & 3];
-        // register-only fast path: no implicit tables, no 'N' list, and per strand either one list with <= 2 codes or two
-        // single-code lists
-#ifdef MKP_NO_FAST_RESOLVE
-        bool fast_read = false;
-#else
-        bool fast_read = !imp_any;
-#endif
-        {
-            uint32_t cnt0 = 0, cnt1 = 0, max0 = 0, max1 = 0;
-            for (uint32_t l2 = 0; l2 < nl; l2++) {
-                if (T.base[l2] == 'N') fast_read = false;
-                if (!T.n_delta[l2]) continue;
-                const uint32_t ncd = T.ncodes[l2];
-                if (T.strand[l2]) { cnt1++; max1 = max(max1, ncd); } else { cnt0++; max0 = max(max0, ncd); }
-            }
-            if (!(cnt0 <= 1 ? max0 <= 2 : (cnt0 == 2 && max0 == 1))) fast_read = false;
-            if (!(cnt1 <= 1 ? max1 <= 2 : (cnt1 == 2 && max1 == 1))) fast_read = false;
-        }
+        const bool fast_read = fast_shape(T, nl, imp_any);
         if (FAST_ONLY && !fast_read) {                 // leave it to the generic instantiation
             if (lane == 0) C.slow_list[atomicAdd(C.work + 4, 1u)] = ri;
             continue;
         }
         RCLK(0);
         RCLK_COUNT(6, 1);
-        // CIGAR prefix: query / reference start of every op; four ops per lane (one 16-byte load), 128 per round
-        const uint32_t nc = h.n_cigar;
-        uint32_t q_total = 0;
-        {
-            uint32_t qc = 0, rc = (uint32_t)h.ref_start;
-            for (uint32_t b = 0; b < nc; b += 128) {
-                const uint32_t i = b + 4 * lane;
-                uint4 c4 = make_uint4(0, 0, 0, 0);
-                if (i < nc) c4 = *(const uint4*)(cig + i);    // 16-byte aligned; words past nc belong to the read's own block
-                const uint32_t cw[4] = {c4.x, c4.y, c4.z, c4.w};
-                uint32_t ql[4], rl[4], qs = 0, rs = 0;
-#pragma unroll
-                for (int k = 0; k < 4; k++) {
-                    const uint32_t c = i + k < nc ? cw[k] : 0u, op = c & 15, len = c >> 4;
-                    ql[k] = (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) ? len : 0;
-                    rl[k] = (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) ? len : 0;
-                    qs += ql[k]; rs += rl[k];
-                }
-                const uint32_t qi = warp_incl_scan(qs), rr = warp_incl_scan(rs);
-                uint32_t q0 = qc + qi - qs, r0 = rc + rr - rs;
-#pragma unroll
-                for (int k = 0; k < 4; k++) {
-                    if (i + k < nc) {
-                        const uint32_t op = cw[k] & 15;
-                        cq[i + k] = 2u * q0 + ((op == 0 || op == 7 || op == 8) ? 1u : 0u);
-                        cr[i + k] = r0;
-                    }
-                    q0 += ql[k]; r0 += rl[k];
-                }
-                qc += __shfl_sync(FULL, qi, 31);
-                rc += __shfl_sync(FULL, rr, 31);
-            }
-            if (lane == 0) cq[nc] = 2u * qc;
-            q_total = qc;
-        }
-        __syncwarp();
+        QueryMap qm;
+        qm.nc = h.n_cigar;
+        qm.cq = h.n_cigar <= CQ_CAP ? s_cq[wib] : gcq;
+        qm.cr = h.n_cigar <= CQ_CAP ? s_cr[wib] : gcr;
+        qm.qt = s_qt[wib];
+        cigar_prefix(qm, cig, (uint32_t)h.ref_start, lane);
         RCLK(1);
-        // query -> op table: qt[t] = the op that holds query base t << shift (the largest i with cq[i] <= that base)
-        uint32_t qt_shift = 7;
-        while (qt_shift < 31 && (q_total >> qt_shift) >= (uint32_t)QT_CAP) qt_shift++;
-        const bool use_qt = nc > 0 && nc <= 65535u;
-        if (use_qt) {
-            const uint32_t B = 1u << qt_shift;
-            for (uint32_t i = lane; i < nc; i += 32) {
-                const uint32_t s0 = cq[i] >> 1, e0 = cq[i + 1] >> 1;
-                for (uint32_t m = (s0 + B - 1) & ~(B - 1); m < e0; m += B) qt[m >> qt_shift] = (uint16_t)i;
-            }
-            if (lane == 0) qt[(q_total + B - 1) >> qt_shift] = (uint16_t)(nc - 1);
-        }
-        __syncwarp();
+        query_op_table(qm, lane);
         RCLK(2);
         uint32_t* P = C.P + meta.entry_off;
         // ---- phase 4: resolve entries -> calls ---------------------------------------------------
@@ -1145,6 +1260,8 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
         uint32_t sum_obs[4] = {0, 0, 0, 0};                    // summary: states seen per canonical base (per lane)
         uint2* calls = C.calls + meta.entry_off;
         if (!err && any_entries) {
+            // (spelled out: through edge_read_ok, ptxas allocates every instantiation differently, and k_resolve<MODE_HIST, false>
+            // spills 8 more bytes each way)
             const bool trim_ok = !c_par.edge_on || !(L <= c_par.edge_start || L <= c_par.edge_end);
             uint32_t skip_mask = 0;       // lists whose every entry sits at the same index of an earlier same-strand list
             for (uint32_t l = 0; l < nl && !err; l++) {
@@ -1184,7 +1301,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                     }
                     if (pp == 2 && (bucket4(c0) != bucket4(pc1) ? (bucket4(pc1) < bucket4(c0)) : (bucket4(c0) == 3))) pp |= 4u;
                     plan = ps | (pp << 4);
-                    base_thr_l = c_par.base_set[tb_l] ? c_par.base_thr[tb_l] : c_par.default_thr;
+                    base_thr_l = base_threshold(tb_l);
                     thr_s0 = mod_threshold(c0, tb_l, base_thr_l);
                     thr_p0 = mod_threshold((pp & 4u) ? pc1 : c0, tb_l, base_thr_l);
                     thr_p1 = mod_threshold((pp & 4u) ? c0 : pc1, tb_l, base_thr_l);
@@ -1328,7 +1445,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                                             uint32_t s0 = 0, s1 = 0;
                                             if (n2c >= 1) { s0 = (uint32_t)state_id(C, scache, tb, k0); mask |= 1u << s0; }
                                             if (n2c == 2) { s1 = (uint32_t)state_id(C, scache, tb, k1); mask |= 1u << s1; }
-                                            const float base_thr = c_par.base_set[tb] ? c_par.base_thr[tb] : c_par.default_thr;
+                                            const float base_thr = base_threshold(tb);
                                             bool have = false;
                                             float best = 0.f;
                                             uint32_t tk = 0, ts = 0;
@@ -1341,7 +1458,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                                             if (!have) tk = 0;
                                             const uint32_t as = (n2c == 2 && p1 >= p0) ? s1 : s0;
                                             const uint32_t ak = (hm2 && mp > cp) ? 2u : 1u;
-                                            ccode = tk | (ts << 2) | (ak << 8) | (as << 10);     // summary record of this value
+                                            ccode = sample_class(tk, ts, ak, as);     // summary record of this value
                                         }
                                     }
                                 }
@@ -1409,7 +1526,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                                         }
                                         const uint32_t ak = (hm && mp2 > cp2) ? 2u : 1u;
                                         if (ak == 2) as = (uint32_t)state_id(C, scache, tb, acode);
-                                        ccode = (uint32_t)tkind | (ts << 2) | (ak << 8) | (as << 10);
+                                        ccode = sample_class((uint32_t)tkind, ts, ak, as);
                                     }
                                 }
                             }
@@ -1417,21 +1534,9 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                             RCLK_MARK;
                             if (!e2) {
                                 bool keep = trim_ok;
-                                if (keep && c_par.edge_on) {
-                                    if (c_par.edge_inv) keep = f < c_par.edge_start || f >= L - c_par.edge_end;
-                                    else keep = f >= c_par.edge_start && f < L - c_par.edge_end;
-                                }
+                                if (keep) keep = edge_keep(f, L);
                                 if (keep) {
-                                    // aligned?  the op holding q = largest i with cq[i] >> 1 <= q, narrowed by the table
-                                    bool aligned = false;
-                                    if (nc > 0 && q < q_total) {
-                                        uint32_t lo = 0, hi = nc;
-                                        if (use_qt) { const uint32_t t = q >> qt_shift; lo = qt[t]; hi = (uint32_t)qt[t + 1] + 1u; }
-                                        const uint32_t key = 2u * q + 1u;
-                                        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (cq[mid] <= key) lo = mid; else hi = mid; }
-                                        const uint32_t e = cq[lo];
-                                        if ((e & 1u) && q < (cq[lo + 1] >> 1)) { aligned = true; rpos = cr[lo] + (q - (e >> 1)); }
-                                    }
+                                    const bool aligned = project(qm, q, rpos);
                                     if (MODE == MODE_PILEUP) {
                                         // (mod strand, read orientation) -> reference strand (read_cache.rs:181-188)
                                         if ((st == 0) != rev) pos_mask |= mask; else neg_mask |= mask;
@@ -1451,7 +1556,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                                                 }
                                             }
                                             emit = true;
-                                            info = st | ((uint32_t)b << 1) | (state << 3) | (nosub << 11);
+                                            info = call_info(st, (uint32_t)b, state, nosub);
                                         }
                                     } else {
                                         bool pass = aligned || C.hist_include_unaligned;
@@ -1484,7 +1589,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                             calls[n_calls + __popc(em & ((1u << lane) - 1u))] = make_uint2(rpos, info);
                             // marks of a read that fails later stay behind: a hot position without calls yields no rows
                             const uint32_t x = rpos - C.cs;
-                            const uint32_t t = (info & 1u) ^ (rev ? 1u : 0u);        // reference strand of the call
+                            const uint32_t t = call_strand(info) ^ (rev ? 1u : 0u);        // reference strand of the call
                             if (!C.list_mode) atomicOr(&C.hot[t * ((C.ce - C.cs + 31) >> 5) + (x >> 5)], 1u << (x & 31));
                         }
                         n_calls += __popc(em);
@@ -1499,7 +1604,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                             uint32_t inexact = ((float)bin != sc || bin < 0 || bin >= MKP_HIST_BINS) ? 1u : 0u;
                             if (bin < 0) bin = 0;
                             if (bin >= MKP_HIST_BINS) bin = MKP_HIST_BINS - 1;
-                            calls[n_hist + __popc(hm & ((1u << lane) - 1u))] = make_uint2((uint32_t)bin | ((uint32_t)hist_base << 16) | (inexact << 20) | (hist_q << 21), __float_as_uint(hist_v));
+                            calls[n_hist + __popc(hm & ((1u << lane) - 1u))] = make_uint2(sample_key((uint32_t)bin, (uint32_t)hist_base, inexact, hist_q), __float_as_uint(hist_v));
                         }
                         n_hist += __popc(hm);
                     }
@@ -1513,81 +1618,9 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
         // ---- phase 4b: implicit tables (every other occurrence of the base is an inferred-canonical entry) ----
         uint32_t imp_meta[2] = {0, 0};
         unsigned long long imp_hist[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-        if (!FAST_ONLY && !err) {
-            const bool trim_ok = !c_par.edge_on || !(L <= c_par.edge_start || L <= c_par.edge_end);
-            for (uint32_t sb = 0; sb < 8; sb++) {
-                const uint32_t s = sb >> 2, b = sb & 3;
-                const uint32_t lists = imp_lists[s][b];
-                if (!lists || !trim_ok) continue;
-                const uint32_t xn = 1u << (rev ? 3 - b : b);          // SEQ nibble of the forward base b
-                // survives the edge filter?  (any occurrence of the base with a kept forward position)
-                bool any = false;
-                for (uint32_t q = lane; q < L && !any; q += 32) {
-                    if (seq_nibble(seq, q) != xn) continue;
-                    const uint32_t f = rev ? L - 1u - q : q;
-                    bool keep = true;
-                    if (c_par.edge_on) keep = c_par.edge_inv ? (f < c_par.edge_start || f >= L - c_par.edge_end) : (f >= c_par.edge_start && f < L - c_par.edge_end);
-                    any = keep;
-                }
-                if (!__any_sync(FULL, any)) continue;
-                Items m, mc;
-                m.n = 0;
-                int ord[MAX_MAP];
-                for (uint32_t l = 0; l < nl; l++) if ((lists >> l) & 1u) for (uint32_t c = 0; c < T.ncodes[l]; c++) if (m.find(T.code[l][c]) < 0) m.push(T.code[l][c], 0.f);
-                iter_order(m, ord);
-                const Items* use = &m;
-                if (c_par.numeric_mode == 2) { redistribute_items(m, ord, c_par.collapse_code, mc); iter_order(mc, ord); use = &mc; }
-                const int tb = s == 0 ? (int)b : 3 - (int)b;
-                table_survived = true;
-                if (MODE == MODE_PILEUP) {
-                    uint32_t mask = 0;
-                    for (int k = 0; k < use->n; k++) mask |= 1u << state_id(C, scache, tb, use->code[k]);
-                    if ((s == 0) != rev) pos_mask |= mask; else neg_mask |= mask;
-                    uint32_t code = 0;
-                    const int kind = make_call_items(*use, ord, tb, &code);
-                    const uint32_t state = kind == 0 ? 0u : kind == 1 ? 1u : 2u + (uint32_t)state_id(C, scache, tb, code);
-                    imp_meta[s] |= (0x80u | state) << (8 * b);
-                } else {
-                    if (C.summ) for (int k = 0; k < use->n; k++) sum_obs[tb] |= 1u << state_id(C, scache, tb, use->code[k]);
-                    // values: argmax of an all-zero map = canonical probability 1.0 for every passing inferred position
-                    unsigned long long n_pass = 0;
-                    if (C.hist_include_unaligned && !C.focus_pos) {
-                        for (uint32_t q = lane; q < L; q += 32) {
-                            if (seq_nibble(seq, q) != xn) continue;
-                            const uint32_t f = rev ? L - 1u - q : q;
-                            bool keep = true;
-                            if (c_par.edge_on) keep = c_par.edge_inv ? (f < c_par.edge_start || f >= L - c_par.edge_end) : (f >= c_par.edge_start && f < L - c_par.edge_end);
-                            if (keep) n_pass++;
-                        }
-                    } else {
-                        uint32_t qc2 = 0, rc2 = (uint32_t)h.ref_start;
-                        const uint32_t* bm = C.focus_pos ? (((s == 0) == rev) ? C.focus_neg : C.focus_pos) : nullptr;
-                        for (uint32_t i = 0; i < h.n_cigar; i++) {
-                            const uint32_t c = cig[i], op = c & 15, len = c >> 4;
-                            if (op == 0 || op == 7 || op == 8) {
-                                for (uint32_t k = lane; k < len; k += 32) {
-                                    const uint32_t q = qc2 + k;
-                                    if (q >= L || seq_nibble(seq, q) != xn) continue;
-                                    const uint32_t f = rev ? L - 1u - q : q;
-                                    bool keep = true;
-                                    if (c_par.edge_on) keep = c_par.edge_inv ? (f < c_par.edge_start || f >= L - c_par.edge_end) : (f >= c_par.edge_start && f < L - c_par.edge_end);
-                                    if (keep && bm) {
-                                        const uint32_t r = rc2 + k;
-                                        keep = r >= C.cs && r < C.ce && ((bm[(r - C.cs) >> 5] >> ((r - C.cs) & 31)) & 1u);
-                                    }
-                                    if (keep) n_pass++;
-                                }
-                            }
-                            if (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) qc2 += len;
-                            if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) rc2 += len;
-                        }
-                    }
-                    n_pass = __reduce_add_sync(FULL, (uint32_t)n_pass);
-                    const uint32_t n_exp = __reduce_add_sync(FULL, imp_explicit[sb]);
-                    imp_hist[sb] = n_pass > n_exp ? n_pass - n_exp : 0;
-                }
-            }
-        }
+        if (!FAST_ONLY && !err)
+            implicit_tables<MODE>(C, scache, T, nl, imp_lists, h, cig, seq, L, rev, lane, imp_explicit, sum_obs, pos_mask, neg_mask,
+                                  table_survived, imp_meta, imp_hist);
         pos_mask = __reduce_or_sync(FULL, pos_mask);
         neg_mask = __reduce_or_sync(FULL, neg_mask);
         table_survived = __any_sync(FULL, table_survived);
@@ -1605,7 +1638,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                     uint32_t qc2 = 0, rc2 = (uint32_t)h.ref_start;
                     for (uint32_t i = 0; i < h.n_cigar; i++) {
                         const uint32_t c = cig[i], op = c & 15, len = c >> 4;
-                        if (op == 0 || op == 7 || op == 8) {
+                        if (cig_is_match(op)) {
                             for (uint32_t k = lane; k < len; k += 32) {
                                 const uint32_t q = qc2 + k, r = rc2 + k;
                                 if (q >= L || r < C.cs || r >= C.ce) continue;
@@ -1614,7 +1647,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                                 const uint32_t b = rev ? 3 - nb : nb;
                                 if (!(((imp_meta[0] | imp_meta[1]) >> (8 * b)) & 0x80u)) continue;
                                 const uint32_t f = rev ? L - 1u - q : q;
-                                if (c_par.edge_on && !(c_par.edge_inv ? (f < c_par.edge_start || f >= L - c_par.edge_end) : (f >= c_par.edge_start && f < L - c_par.edge_end))) continue;
+                                if (!edge_keep(f, L)) continue;
                                 const uint32_t x = r - C.cs;
                                 if (C.focus_pos && !(((C.focus_pos[x >> 5] | C.focus_neg[x >> 5]) >> (x & 31)) & 1u)) continue;
                                 // the table of mod strand s counts on reference strand s ^ rev
@@ -1623,8 +1656,8 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                                     if ((imp_meta[s] >> (8 * b)) & 0x80u) atomicOr(&C.hot[(s ^ (rev ? 1u : 0u)) * nw + (x >> 5)], 1u << (x & 31));
                             }
                         }
-                        if (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) qc2 += len;
-                        if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) rc2 += len;
+                        qc2 += cig_qlen(op, len);
+                        rc2 += cig_rlen(op, len);
                     }
                 }
             }
@@ -1637,7 +1670,7 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                     uint32_t seen = 0;
                     for (uint32_t k = lane; k < n_hist; k += 32) {
                         const uint2 v = calls[k];
-                        const uint32_t tb = (v.x >> 16) & 3u, tk = v.y & 3u, ts = (v.y >> 2) & 63u, ak = (v.y >> 8) & 3u, as = (v.y >> 10) & 63u;
+                        const uint32_t tb = sample_base(v.x), tk = class_tkind(v.y), ts = class_tstate(v.y), ak = class_akind(v.y), as = class_astate(v.y);
                         seen |= 1u << tb;
                         // pass: the thresholded call; fail: filed under the arg-max call (src/summarize.rs:186-214)
                         if (tk == 1) atomicAdd(&C.summ[(tb * 2 + 0) * 33 + 0], 1ull);
@@ -1650,10 +1683,9 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                     for (int b = 0; b < 4; b++) obs[b] = __reduce_or_sync(FULL, sum_obs[b]);
                     if (lane == 0) {
                         for (int sb = 0; sb < 8; sb++) if (imp_hist[sb]) {
-                            const int tb = (sb >> 2) == 0 ? (sb & 3) : 3 - (sb & 3);
+                            const int tb = table_base(sb);
                             // an inferred entry is the all-zero map: canonical with probability 1.0
-                            const float base_thr = c_par.base_set[tb] ? c_par.base_thr[tb] : c_par.default_thr;
-                            atomicAdd(&C.summ[(tb * 2 + (1.0f >= base_thr ? 0 : 1)) * 33 + 0], imp_hist[sb]);
+                            atomicAdd(&C.summ[(tb * 2 + (1.0f >= base_threshold(tb) ? 0 : 1)) * 33 + 0], imp_hist[sb]);
                             seen |= 1u << tb;
                         }
                         for (int b = 0; b < 4; b++) {
@@ -1665,23 +1697,23 @@ __global__ void __launch_bounds__(128, FAST_ONLY ? MKP_MINB_RESOLVE_FAST : MKP_M
                 if (C.qhist) {
                     for (uint32_t k = lane; k < n_hist; k += 32) {
                         const uint2 v = calls[k];
-                        const uint32_t tb = (v.x >> 16) & 3u, q = (v.x >> 21) & 255u, ak = (v.y >> 8) & 3u, as = (v.y >> 10) & 63u;
+                        const uint32_t tb = sample_base(v.x), q = sample_qual(v.x), ak = class_akind(v.y), as = class_astate(v.y);
                         atomicAdd(&C.qhist[(tb * 33 + (ak == 2 ? 1 + as : 0)) * 256 + q], 1ull);
                     }
                     // an inferred entry is the all-zero map: canonical with probability 1.0, qual 255
                     if (lane == 0) for (int sb = 0; sb < 8; sb++) if (imp_hist[sb]) {
-                        const int tb = (sb >> 2) == 0 ? (sb & 3) : 3 - (sb & 3);
+                        const int tb = table_base(sb);
                         atomicAdd(&C.qhist[(tb * 33 + 0) * 256 + 255], imp_hist[sb]);
                     }
                 }
                 if (C.hist) {
                     for (uint32_t k = lane; k < n_hist; k += 32) {
                         uint32_t v = calls[k].x;
-                        atomicAdd(&C.hist[((v >> 16) & 3u) * MKP_HIST_BINS + (v & 0xffffu)], 1ull);
-                        if ((v >> 20) & 1u) atomicAdd(C.hist_inexact, 1ull);
+                        atomicAdd(&C.hist[sample_base(v) * MKP_HIST_BINS + sample_bin(v)], 1ull);
+                        if (sample_inexact(v)) atomicAdd(C.hist_inexact, 1ull);
                     }
                     if (lane == 0) for (int sb = 0; sb < 8; sb++) if (imp_hist[sb]) {
-                        const int tb = (sb >> 2) == 0 ? (sb & 3) : 3 - (sb & 3);
+                        const int tb = table_base(sb);
                         atomicAdd(&C.hist[tb * MKP_HIST_BINS + 1024u], imp_hist[sb]);
                     }
                 }
@@ -1789,7 +1821,7 @@ __global__ void __launch_bounds__(256) k_items_count(const mkp_read_hdr* __restr
     uint32_t rc = (uint32_t)h.ref_start;
     for (uint32_t b0 = 0; b0 < h.n_cigar && rc < ce; b0 += 32) {      // (the part past the chunk end is not needed)
         const uint32_t i = b0 + lane, c = i < h.n_cigar ? cig[i] : 0, op = c & 15;
-        rc += __reduce_add_sync(FULL, (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) ? c >> 4 : 0u);
+        rc += __reduce_add_sync(FULL, cig_rlen(op, c >> 4));
     }
     const uint32_t lo = (uint32_t)h.ref_start > cs ? (uint32_t)h.ref_start : cs, hi = rc < ce ? rc : ce;
     if (lane == 0) n_items[ri] = lo < hi ? count_items_of(lo - cs, hi - cs, S) : 0u;
@@ -1810,8 +1842,7 @@ __global__ void __launch_bounds__(256) k_items_fill(const mkp_read_hdr* __restri
     uint32_t qc = 0, rc = (uint32_t)h.ref_start;
     for (uint32_t b0 = 0; b0 < h.n_cigar && rc <= last; b0 += 32) {
         const uint32_t i = b0 + lane, c = i < h.n_cigar ? cig[i] : 0, op = c & 15, len = c >> 4;
-        const uint32_t ql = (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) ? len : 0;
-        const uint32_t rl = (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) ? len : 0;
+        const uint32_t ql = cig_qlen(op, len), rl = cig_rlen(op, len);
         const uint32_t qi = warp_incl_scan(ql), rr = warp_incl_scan(rl);
         const uint32_t q0 = qc + qi - ql, r0 = rc + rr - rl, e = r0 + rl;
         qc += __shfl_sync(FULL, qi, 31);
@@ -1895,7 +1926,7 @@ __global__ void __launch_bounds__(256) k_count_calls(CountDev D) {
             uint2 c = calls[k];
             uint32_t x = c.x - D.cs;
             uint32_t info = c.y;
-            uint32_t st = info & 1u, b = (info >> 1) & 3u, state = (info >> 3) & 0xffu, nosub = (info >> 11) & 1u;
+            const uint32_t st = call_strand(info), b = call_base(info), state = call_state(info), nosub = call_nosub(info);
             const uint4 r = D.rec[x >> 5];                     // (a pair outside the focus set has no slot)
             const uint32_t bit = x & 31, t = st == 0 ? a : 1u - a, pbb = st == 0 ? b : 3u - b;
             // cancel what k_count_bases adds for this (read, position): the inferred entry of this table if the
@@ -1999,8 +2030,7 @@ __global__ void __launch_bounds__(256, MKP_MINB_BASES) k_count_bases(CountDev D)
             uint32_t i = b0 + lane;
             uint32_t c = i < h.n_cigar ? cig[i] : 0;
             uint32_t op = c & 15, len = c >> 4;
-            uint32_t ql = (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) ? len : 0;
-            uint32_t rl = (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) ? len : 0;
+            uint32_t ql = cig_qlen(op, len), rl = cig_rlen(op, len);
             uint32_t qi = warp_incl_scan(ql), rr = warp_incl_scan(rl);
             uint32_t q0 = qc + qi - ql, r0 = rc + rr - rl;
             qc += __shfl_sync(FULL, qi, 31);
@@ -2046,7 +2076,7 @@ __global__ void __launch_bounds__(256, MKP_MINB_BASES) k_count_bases(CountDev D)
                                 if ((rel >> 5) >= wt) atomicOr(&s_mask[wib][(rel >> 5) - wt], 1u << (rel & 31));
 #ifndef MKP_NO_FUSED_CALLS
                                 // the record's own counter (k_count_calls leaves these reads alone): modcall / canonical / filtered
-                                const uint32_t st = info & 1u, cb = (info >> 1) & 3u, state = (info >> 3) & 0xffu;
+                                const uint32_t st = call_strand(info), cb = call_base(info), state = call_state(info);
                                 add_feature(D.slots, D.stride, D.rec[rel >> 5], rel & 31, st == 0 ? a : 1u - a, st == 0 ? cb : 3u - cb, state, 1u);
 #endif
                             }
@@ -2084,7 +2114,7 @@ __global__ void __launch_bounds__(256, MKP_MINB_BASES) k_count_bases(CountDev D)
                         const uint32_t r = wbase + bit;
                         while (s_r[wib][j + 1] <= r) j++;
                         const uint32_t jc = s_op[wib][j], jop = jc & 15;
-                        if (!(jop == 0 || jop == 7 || jop == 8 || jop == 2)) continue;       // reference skip
+                        if (!(cig_is_match(jop) || jop == 2)) continue;       // reference skip
                         if (jop == 2 && !((ok >> bit) & 1u)) continue;
                         uint32_t* S = D.slots + (size_t)(pre + __popc(ok & ((1u << bit) - 1u))) * D.stride;   // (when ok has the bit)
                         if (jop == 2) { atomicAdd(&S[SL_DEL], 1u); continue; }
@@ -2097,7 +2127,7 @@ __global__ void __launch_bounds__(256, MKP_MINB_BASES) k_count_bases(CountDev D)
                         if ((ip | in) & 0x80u) {
                             // inferred-canonical entries of implicit tables, subject to the edge filter
                             const uint32_t f = a ? h.l_seq - 1u - q : q;
-                            if (c_par.edge_on && !(c_par.edge_inv ? (f < c_par.edge_start || f >= h.l_seq - c_par.edge_end) : (f >= c_par.edge_start && f < h.l_seq - c_par.edge_end))) ip = in = 0;
+                            if (!edge_keep(f, h.l_seq)) ip = in = 0;
                         }
                         if (!((ip | in) & 0x80u)) { if ((ok >> bit) & 1u) atomicAdd(&S[SL_BASE + b], 1u); continue; }
                         if (ip & 0x80u) add_feature(D.slots, D.stride, wr, bit, a, b, ip & 0x7fu, 1u);
@@ -2263,8 +2293,7 @@ __global__ void __launch_bounds__(128) k_hemi_count(HemiDev D) {
             for (uint32_t b0 = 0; b0 < nc; b0 += 32) {
                 const uint32_t i = b0 + lane;
                 const uint32_t c = i < nc ? cig[i] : 0u, op = c & 15, len = c >> 4;
-                const uint32_t ql = (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) ? len : 0;
-                const uint32_t rl = (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) ? len : 0;
+                const uint32_t ql = cig_qlen(op, len), rl = cig_rlen(op, len);
                 const uint32_t qi = warp_incl_scan(ql), rr = warp_incl_scan(rl);
                 if (i < nc) { cq[i] = qc + qi - ql; cr[i] = rc + rr - rl; }
                 qc += __shfl_sync(FULL, qi, 31);
@@ -2294,7 +2323,7 @@ __global__ void __launch_bounds__(128) k_hemi_count(HemiDev D) {
             while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (cr[mid] <= r) lo = mid; else hi = mid; }
             const uint32_t c = cig[lo], op = c & 15, len = c >> 4;
             if (r >= cr[lo] + len) return 0;
-            if (op == 0 || op == 7 || op == 8) { *q = cq[lo] + (r - cr[lo]); return *q < h.l_seq ? 1u : 0u; }
+            if (cig_is_match(op)) { *q = cq[lo] + (r - cr[lo]); return *q < h.l_seq ? 1u : 0u; }
             return op == 2 ? 2u : 0u;
         };
         // the read's call at r on mod strand st, forward base cb: state + 1 (1 filtered, 2 canonical, 3 + id), 0 = none
@@ -2306,14 +2335,14 @@ __global__ void __launch_bounds__(128) k_hemi_count(HemiDev D) {
                 for (uint32_t k = lo; k < end; k++) {
                     const uint2 c = rcalls[k];
                     if (c.x != r) break;
-                    if ((c.y & 1u) == st && ((c.y >> 1) & 3u) == cb) return ((c.y >> 3) & 0xffu) + 1u;
+                    if (call_strand(c.y) == st && call_base(c.y) == cb) return call_state(c.y) + 1u;
                 }
             }
             // implicit table: every other occurrence of its base is an inferred-canonical entry, subject to the edge filter
             const uint32_t imp = (m.imp[st] >> (8 * cb)) & 0xffu;
             if (!(imp & 0x80u)) return 0;
             const uint32_t f = a ? h.l_seq - 1u - q : q;
-            if (c_par.edge_on && !(c_par.edge_inv ? (f < c_par.edge_start || f >= h.l_seq - c_par.edge_end) : (f >= c_par.edge_start && f < h.l_seq - c_par.edge_end))) return 0;
+            if (!edge_keep(f, h.l_seq)) return 0;
             return (imp & 0x7fu) + 1u;
         };
         if (lo_r >= hi_r) continue;
